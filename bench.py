@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- encoder input MB/s of the Brotli hot path on B200 (BASELINE.json metric "q5/q9").
+"""bench.py -- encoder input MB/s of the Brotli hot path on H100 (BASELINE.json metric "q5/q9").
 
 One JSON line.  The HEADLINE keys (value / e2e / roofline / cpu_baseline) are BASELINE.json configs[1]:
 every rank compresses its own 100 000 000-byte enwik8-shaped text stream at quality 5, lgwin 22
@@ -15,9 +15,8 @@ metric, each with its own value / e2e / roofline / cpu_baseline / bit_exact:
       GPU j mod N (strong scaling), one device batch per rank
   c5q5  c5's streams at quality 5 (many small web payloads as device jobs; not a BASELINE config)
   q234  the headline's 100 MB text at quality 2, 3 and 4 plus 2 000 x 64 KiB web payloads at quality 2 and 4
-      (SURVEY.md 8f rank 1; not a BASELINE config; N = 1 only).  The path was built after the round's last GPU
-      minute, so it runs LAST and in a CHILD PROCESS with a time limit: whatever it does on its first contact with
-      hardware, the headline line is printed.
+      (SURVEY.md 8f rank 1; not a BASELINE config; N = 1 only).  It runs LAST and in a CHILD PROCESS with a time
+      limit: whatever happens to it, the headline line is printed.
 
 Per config:  value = whole-job input MB/s, inputs resident in HBM, shards gathered to rank 0 in the step;
 e2e = the same from HOST buffers: H2D of the inputs and D2H of the compressed bytes inside the timed region
@@ -28,7 +27,14 @@ reference (oracle/_ref) run on the box's CPU on the same bytes, by every rank fo
 
   --impl reference : the reference's own CPU encoder (oracle/_ref; falls back to the oracle port) timed on
                      the host cores on the same configs; rank 0 only.
-  --configs c2,c4  : subset (the headline c2 always runs).
+  --configs c2,c4,c3,c5,c5q5,q234 : the sub-results to add (the headline c2 always runs).  By default only the headline
+                     runs: with every config taking K steps the whole set, and its CPU parity checks (200 MB at quality 9
+                     alone takes minutes on one core), runs far beyond ten minutes on one H100.
+  --steps K / --warmup W : timed and warm-up steps of every config that runs.
+  --dump-outputs DIR : after the timed steps, write what the last timed step of each config returned (rank 0's share)
+                     to DIR as <config>_bytes.npy (the compressed bytes as float32; above 2^20 bytes a fixed seeded sample
+                     of 2^20 positions, ascending) and <config>_sizes.npy (the compressed size of every stream, float64).
+                     The inputs are generated from fixed seeds, so two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -54,13 +60,14 @@ WORKLOADS = {
     "c5": "10 000 x 64 KiB streams (slices of the c3 mix at offsets i*104729 mod (2^30-65536)), quality 1, lgwin 22, stream j on GPU j mod N",
     "c5q5": "c5's 10 000 x 64 KiB streams at quality 5, lgwin 22 (many small web payloads; not a BASELINE config), stream j on GPU j mod N",
     "q234": "c2's 100 MB text at quality 2, 3 and 4, lgwin 22 (SURVEY 8f rank 1; not a BASELINE config), N = 1 only, run in a child "
-            "process with a time limit so that this newest path cannot take the headline line with it",
+            "process with a time limit so that it cannot take the headline line with it",
 }
 QL = {"c2": (5, 22), "c3": (5, 22), "c4": (9, 24), "c5": (1, 22), "c5q5": (5, 22), "q234": (4, 22)}
 METRIC = "encoder input MB/s (bit-exact)"
-# the headline's config: identical in both arms (the driver compares them)
+# the headline's config: identical in both arms (--impl b200 and --impl reference)
 HEAD_CONFIG = {"workload": WORKLOADS["c2"], "quality": 5, "lgwin": 22, "input_bytes_per_gpu": C2_BYTES,
-               "l2": "no L2 flush needed: every step streams the 100 MB input and a ~3.5 GB index, far beyond the 126 MB L2"}
+               "l2": "no L2 flush needed: every step streams the 100 MB input and a ~3.5 GB index, far beyond the 50 MB L2"}
+DUMP_BYTES = 1 << 20
 
 
 def log(*a):
@@ -212,24 +219,26 @@ def run_reference(args, rank):
             d0 = make_stream_input("c2", 0, 1)
             per = {}
             for q in (2, 3, 4):
-                t0 = time.time(); lib.compress(d0, q, 22); dt = time.time() - t0
-                per["q%d" % q] = {"value": round(len(d0) / dt / 1e6, 2), "unit": "MB/s", "ms_per_step": round(1e3 * dt, 2), "steps": 1,
+                for _ in range(args.warmup):
+                    lib.compress(d0, q, 22)
+                t0 = time.time()
+                for _ in range(args.steps):
+                    lib.compress(d0, q, 22)
+                dt = (time.time() - t0) / args.steps
+                per["q%d" % q] = {"value": round(len(d0) / dt / 1e6, 2), "unit": "MB/s", "ms_per_step": round(1e3 * dt, 2),
+                                  "steps": args.steps, "warmup": args.warmup,
                                   "e2e": {"value": round(len(d0) / dt / 1e6, 2), "unit": "MB/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
                                   "cpu_baseline": {"value": round(len(d0) / dt / 1e6, 2), "unit": "MB/s", "cores": 1, "kind": kind,
-                                                   "sample": "the whole %d-byte stream once, 1 thread" % len(d0)}}
+                                                   "sample": "the whole %d-byte stream per step, 1 thread" % len(d0)}}
             line["sub_results"][cfg] = {"workload": WORKLOADS[cfg], "lgwin": 22, "per_quality": per}
             continue
-        v, ms, cores, sample = reference_config(cfg, lib, args.gpus, 1, 0)
+        v, ms, cores, sample = reference_config(cfg, lib, args.gpus, args.steps, args.warmup)
         line["sub_results"][cfg] = {"workload": WORKLOADS[cfg], "quality": QL[cfg][0], "lgwin": QL[cfg][1],
-                                    "value": round(v, 2), "unit": "MB/s", "ms_per_step": round(ms, 2), "steps": 1,
+                                    "value": round(v, 2), "unit": "MB/s", "ms_per_step": round(ms, 2),
+                                    "steps": args.steps, "warmup": args.warmup,
                                     "cpu_baseline": {"value": round(v, 2), "unit": "MB/s", "cores": cores, "kind": kind, "sample": sample},
                                     "e2e": {"value": round(v, 2), "unit": "MB/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     _emit(line)
-
-
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed ncu captures
-# (profiles/): k_walk's first launch on c2, k_q1_parse on c5.  None where no capture of that config exists.
-TRAFFIC_GB = {"c2": 13.35, "c5": 114.0}   # profiles/r02u_summary.md (k_walk<1>), profiles/r01i_summary.md (k_q1_parse)
 
 
 _REAL_STDOUT = None
@@ -265,7 +274,29 @@ def hbm_peak():
         v = json.load(open(p)).get("hbm_gbs")
         if v:
             return float(v), "MEASURED_PEAKS.json hbm_gbs (measured copy bandwidth)"
-    return 6550.0, "fallback of /opt/skills/guides/B200_PROFILING.md (MEASURED_PEAKS.json absent)"
+    return 3350.0, "NVIDIA H100 SXM data sheet HBM3 bandwidth (MEASURED_PEAKS.json absent)"
+
+
+def gpu_info():
+    """The card the numbers were measured on and its power limit (a power-limited card runs lower clocks)."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", os.environ.get("LOCAL_RANK", "0"), "--query-gpu=name,power.limit",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=10).stdout
+        name, limit = [x.strip() for x in out.strip().split(",")[:2]]
+        return {"name": name, "power_limit_w": float(limit)}
+    except Exception:
+        return {"name": None, "power_limit_w": None}
+
+
+def dump_output(dump_dir, name, data, sizes):
+    """--dump-outputs: `data` (compressed bytes, a sample of DUMP_BYTES fixed positions above that) and `sizes`."""
+    import numpy as np
+    a = np.frombuffer(bytes(data), np.uint8)
+    if a.size > DUMP_BYTES:
+        a = a[np.sort(np.random.default_rng(0).choice(a.size, DUMP_BYTES, replace=False))]
+    os.makedirs(dump_dir, exist_ok=True)
+    np.save(os.path.join(dump_dir, name + "_bytes.npy"), a.astype(np.float32))
+    np.save(os.path.join(dump_dir, name + "_sizes.npy"), np.asarray(sizes, np.float64))
 
 
 def bench_stream(ctx, cfg, steps, warmup, extra_warm=True):
@@ -317,6 +348,8 @@ def bench_stream(ctx, cfg, steps, warmup, extra_warm=True):
     dt, outs = ctx.timed(step_device, steps)
     st = brotli_b200.last_stats()
     out_size = outs[-1]
+    if ctx.dump and rank == 0:
+        dump_output(ctx.dump, cfg, d_out[:out_size].cpu().numpy(), [out_size])
     if world == 1:
         if extra_warm:
             step_e2e_c_abi(h_in, h_out)
@@ -378,9 +411,7 @@ def bench_stream(ctx, cfg, steps, warmup, extra_warm=True):
         algo = st["walk_bytes"] * (1.0 + out_size / float(n))
         ach = algo / (walk_ms / 1e3) / 1e9
         r["roofline"] = {"bound": "hbm", "kernel": "k_walk", "achieved": round(ach, 3), "peak": peak, "unit": "GB/s",
-                         "frac": round(ach / peak, 6), "traffic": TRAFFIC_GB.get(cfg),
-                         "traffic_unit": "GB of DRAM read+write per launch (ncu --set full, profiles/)",
-                         "algorithmic_gb": round(algo / 1e9, 4), "kernel_ms": round(walk_ms, 2),
+                         "frac": round(ach / peak, 6), "algorithmic_gb": round(algo / 1e9, 4), "kernel_ms": round(walk_ms, 2),
                          "launches": int(st["walk_launches"]), "peak_source": src}
     if world == 1:
         r["cpu_baseline"] = {"value": round(n / t_cpu / 1e6, 2), "unit": "MB/s", "cores": 1, "kind": kind,
@@ -452,6 +483,8 @@ def bench_c5(ctx, steps, warmup):
     dt, outs = ctx.timed(step_device, steps)
     st = brotli_b200.last_stats_q1()
     dense = outs[-1]
+    if ctx.dump and rank == 0:
+        dump_output(ctx.dump, "c5", d_out[:dense].cpu().numpy(), [int(out_sz[k]) for k in range(cnt)])
     step_e2e()
     dt_e2e, _ = ctx.timed(step_e2e, steps)
     out_total = sum(int(out_sz[k]) for k in range(cnt))
@@ -492,9 +525,7 @@ def bench_c5(ctx, steps, warmup):
                           "path": "BrotliB200CompressBatch(host pointer arrays, pageable per-stream buffers) incl. ctypes marshalling, one call per rank"},
          "stages_ms": {k: round(st[k], 2) for k in ("ms_total", "ms_h2d", "ms_parse", "ms_code", "ms_pack", "ms_d2h")},
          "roofline": {"bound": "hbm", "kernel": "k_q1_parse", "achieved": round(ach, 3), "peak": peak, "unit": "GB/s",
-                      "frac": round(ach / peak, 6), "traffic": TRAFFIC_GB.get("c5") if world == 1 else None,
-                      "traffic_unit": "GB of DRAM read+write per launch (ncu --set full, profiles/)",
-                      "algorithmic_gb": round(algo / 1e9, 4), "kernel_ms": round(parse_ms, 2), "launches": 1, "peak_source": src},
+                      "frac": round(ach / peak, 6), "algorithmic_gb": round(algo / 1e9, 4), "kernel_ms": round(parse_ms, 2), "launches": 1, "peak_source": src},
          "gpu_launches": int(st["launches"]) * steps}
     if world == 1:
         r["cpu_baseline"] = {"value": round(nbytes / t_cpu_all / 1e6, 2), "unit": "MB/s", "cores": ncpu, "kind": kind,
@@ -534,6 +565,8 @@ def bench_c5q5(ctx, steps, warmup):
     dt, _ = ctx.timed(step, steps)
     st = brotli_b200.last_stats()
     out_total = sum(out_sizes[k] for k in range(cnt))
+    if ctx.dump and rank == 0:
+        dump_output(ctx.dump, "c5q5", b"".join(outs[k].raw[:out_sizes[k]] for k in range(cnt)), [out_sizes[k] for k in range(cnt)])
     kind, lib = ref_lib()
     ncpu = max(1, (os.cpu_count() or 1) // world)
     want = [None] * cnt
@@ -568,7 +601,7 @@ def bench_c5q5(ctx, steps, warmup):
     return r
 
 
-def q234_child():
+def q234_child(steps, warmup, dump):
     """Child process of the q234 sub-result: C2's input at quality 2, 3, 4 on cuda:0; prints one JSON object."""
     import torch
     import brotli_b200
@@ -595,13 +628,15 @@ def q234_child():
             sz = C.c_size_t(cap)
             assert L.BrotliEncoderCompress(q, 22, 0, n, h_in.data_ptr(), C.byref(sz), h_out.data_ptr()), "BrotliEncoderCompress failed"
             return sz.value
-        steps = 3
-        dev(); dev(); dev()                       # W = 3 warm-up steps
+        for _ in range(warmup):
+            dev()
         torch.cuda.synchronize(); t0 = time.perf_counter()
         for _ in range(steps):
             out_size = dev()
         torch.cuda.synchronize(); dt = time.perf_counter() - t0
         st = brotli_b200.last_stats()
+        if dump:
+            dump_output(dump, "q234_q%d" % q, d_out[:out_size].cpu().numpy(), [out_size])
         e2e()
         torch.cuda.synchronize(); t0 = time.perf_counter()
         for _ in range(steps):
@@ -609,7 +644,7 @@ def q234_child():
         torch.cuda.synchronize(); dt2 = time.perf_counter() - t0
         got = bytes(h_out[:out_size].numpy().tobytes())
         t1 = time.time(); want = lib.compress(data, q, 22); t_cpu = time.time() - t1
-        r = {"quality": q, "lgwin": 22, "steps": steps, "warmup": 3, "input_bytes": n, "compressed_bytes": out_size,
+        r = {"quality": q, "lgwin": 22, "steps": steps, "warmup": warmup, "input_bytes": n, "compressed_bytes": out_size,
              "bit_exact": got == want, "value": round(n * steps / dt / 1e6, 2), "unit": "MB/s", "ms_per_step": round(1e3 * dt / steps, 2),
              "e2e": {"value": round(n * steps / dt2 / 1e6, 2), "unit": "MB/s", "h2d_bytes_per_step": n, "d2h_bytes_per_step": out_size,
                      "path": "BrotliEncoderCompress(host in, host out), pinned buffers"},
@@ -651,12 +686,16 @@ def q234_child():
                 C.memmove(out_sizes, caps_arr, C.sizeof(caps_arr))
                 good = L.BrotliB200CompressBatch(q, 22, cnt, in_ptrs, sizes, out_ptrs, out_sizes, 16)
                 assert good == cnt, "BrotliB200CompressBatch: %d of %d" % (good, cnt)
-            step(); step(); step()
+            for _ in range(warmup):
+                step()
             torch.cuda.synchronize(); t0 = time.perf_counter()
-            for _ in range(3):
+            for _ in range(steps):
                 step()
             torch.cuda.synchronize(); dt = time.perf_counter() - t0
             st = brotli_b200.last_stats()
+            if dump:
+                dump_output(dump, "q234_batch_q%d" % q, b"".join(outs[k].raw[:out_sizes[k]] for k in range(cnt)),
+                            [out_sizes[k] for k in range(cnt)])
             want = [None] * cnt
             t1 = time.time()
             def work(k):
@@ -664,10 +703,10 @@ def q234_child():
                     want[i] = lib.compress(streams[i], q, 22)
             run_threads(ncpu, work)
             t_cpu = time.time() - t1
-            v = round(cnt * C5_SIZE * 3 / dt / 1e6, 2)
-            batch["q%d" % q] = {"streams": cnt, "stream_bytes": C5_SIZE, "quality": q, "lgwin": 22, "steps": 3, "warmup": 3,
+            v = round(cnt * C5_SIZE * steps / dt / 1e6, 2)
+            batch["q%d" % q] = {"streams": cnt, "stream_bytes": C5_SIZE, "quality": q, "lgwin": 22, "steps": steps, "warmup": warmup,
                                 "bit_exact": all(outs[k].raw[:out_sizes[k]] == want[k] for k in range(cnt)),
-                                "value": v, "unit": "MB/s", "ms_per_step": round(1e3 * dt / 3, 2),
+                                "value": v, "unit": "MB/s", "ms_per_step": round(1e3 * dt / steps, 2),
                                 "e2e": {"value": v, "unit": "MB/s", "h2d_bytes_per_step": cnt * C5_SIZE,
                                         "d2h_bytes_per_step": sum(out_sizes[k] for k in range(cnt)),
                                         "path": "BrotliB200CompressBatch(host pointer arrays): value == e2e for this call"},
@@ -682,10 +721,11 @@ def q234_child():
     sys.stdout.flush()
 
 
-def bench_q234():
-    """Runs q234_child in a process of its own (time limit 5 minutes; it needs about two): a crash or a hang of the newest
-    path ends the child, not the bench."""
-    p = subprocess.run([sys.executable, os.path.abspath(__file__), "--q234-child"], stdout=subprocess.PIPE, timeout=300)
+def bench_q234(steps, warmup, dump):
+    """Runs q234_child in a process of its own (time limit 5 minutes plus 10 s per step): a crash or a hang of this path
+    ends the child, not the bench."""
+    cmd = [sys.executable, os.path.abspath(__file__), "--q234-child", str(steps), str(warmup)] + ([dump] if dump else [])
+    p = subprocess.run(cmd, stdout=subprocess.PIPE, timeout=300 + 10 * (steps + warmup))
     lines = [l for l in p.stdout.decode("utf-8", "replace").splitlines() if l.startswith("{")]
     if p.returncode != 0 or not lines:
         raise RuntimeError("q234 child exited with %d" % p.returncode)
@@ -694,7 +734,8 @@ def bench_q234():
 
 def main():
     if "--q234-child" in sys.argv:
-        q234_child()
+        a = sys.argv[sys.argv.index("--q234-child") + 1:]
+        q234_child(int(a[0]), int(a[1]), a[2] if len(a) > 2 else None)
         return
     _claim_stdout()
     ap = argparse.ArgumentParser()
@@ -702,7 +743,8 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200")
-    ap.add_argument("--configs", default="c2,c4,c3,c5,c5q5,q234")
+    ap.add_argument("--configs", default="c2")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR")
     args = ap.parse_args()
     args.configs = [c for c in args.configs.split(",") if c in WORKLOADS]
     rank = int(os.environ.get("RANK", "0"))
@@ -722,6 +764,7 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     ctx = Ctx()
     ctx.L, ctx.rank, ctx.world = brotli_b200.lib(), rank, world
+    ctx.dump = os.path.abspath(args.dump_outputs) if args.dump_outputs else None
 
     def barrier():
         torch.cuda.synchronize()
@@ -759,15 +802,15 @@ def main():
         t0 = time.time()
         try:
             if cfg == "c4":
-                sub[cfg] = bench_stream(ctx, "c4", 1, 1, extra_warm=False)
+                sub[cfg] = bench_stream(ctx, "c4", args.steps, args.warmup, extra_warm=False)
             elif cfg == "c3":
-                sub[cfg] = bench_stream(ctx, "c3", 3, 1, extra_warm=False)
+                sub[cfg] = bench_stream(ctx, "c3", args.steps, args.warmup, extra_warm=False)
             elif cfg == "c5":
-                sub[cfg] = bench_c5(ctx, 5, 2)
+                sub[cfg] = bench_c5(ctx, args.steps, args.warmup)
             elif cfg == "c5q5":
-                sub[cfg] = bench_c5q5(ctx, 5, 2)
+                sub[cfg] = bench_c5q5(ctx, args.steps, args.warmup)
             elif cfg == "q234" and world == 1:
-                sub[cfg] = bench_q234()
+                sub[cfg] = bench_q234(args.steps, args.warmup, ctx.dump)
         except Exception as e:      # a sub-result must not take the headline line with it (one rank: the others would hang)
             if world > 1:
                 raise
@@ -779,7 +822,7 @@ def main():
                 "warmup": args.warmup, "ms_per_step": head["ms_per_step"], "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": "u8", "data": "synthetic",
                 "config": HEAD_CONFIG, "bit_exact_vs_reference": head["bit_exact"], "compressed_bytes": head["compressed_bytes"],
-                "clocks": sampler.summary(), "e2e": head["e2e"], "gpu_launches": head["gpu_launches"],
+                "gpu": gpu_info(), "clocks": sampler.summary(), "e2e": head["e2e"], "gpu_launches": head["gpu_launches"],
                 "roofline": head.get("roofline"), "cpu_baseline": head.get("cpu_baseline"),
                 "stages_ms": head["stages_ms"], "lz77": head["lz77"], "host_cores": os.cpu_count(),
                 "sub_results": sub}

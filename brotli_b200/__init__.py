@@ -1,4 +1,4 @@
-"""brotli_b200 -- Python face of libbrotlienc_b200.so (B200-native Brotli encoder hot path).
+"""brotli_b200 -- Python face of libbrotlienc_b200.so (GPU-native Brotli encoder hot path for the H100).
 
 Mirrors the encoder half of the reference's Python module (python/brotli.py:24-49,
 python/_brotli.c:403-458): ``compress()`` and ``Compressor.process/flush/finish`` with the same

@@ -7,7 +7,7 @@
 //   quality 2  BrotliBuildAndStoreHuffmanTreeFast (:404; br_q1.h br_q1_fast_tree, shared with quality 1), or -- for at
 //              most 128 commands -- the static command / distance codes of entropy_encode_static.h with their
 //              pre-serialised forms (:524 StoreStaticCommandHuffmanTree, :538 StoreStaticDistanceHuffmanTree).
-// The B200 shape: one CTA per metablock (k_prep_flat) builds the three histograms with atomics, one thread builds and
+// The GPU shape: one CTA per metablock (k_prep_flat) builds the three histograms with atomics, one thread builds and
 // stores the codes behind the header; the symbols themselves go through the shared, fully data-parallel
 // stages E5 / E6 (br_entropy2.h: per-symbol bit counts -> prefix sums -> atomic-OR scatter), which read this
 // metablock's codes from BrMbFlat.

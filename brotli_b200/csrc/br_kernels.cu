@@ -1,4 +1,4 @@
-// br_kernels.cu -- CUDA kernels (sm_100a) and the per-stream pipeline that drives them.
+// br_kernels.cu -- CUDA kernels (sm_90a) and the per-stream pipeline that drives them.
 //
 // Stage map (reference function -> kernel):
 //   hash keys / bucket rings (hash_longest_match64_inc.h Store*)  -> k_hash_keys, k_radix_* (the last pass writes rank[]), k_seg
@@ -216,8 +216,8 @@ __global__ void __launch_bounds__(1024) k_build_storedS(BrStream s, u32* __restr
 #endif
 #ifndef BR_WALK_G_DEEP
 #define BR_WALK_G_DEEP 4    /* rows fetched together for the 256-entry rings of quality 9: 8 (the whole ring, 125 registers,
-                               16 warps per SM) walks one chunk faster, 4 (96 registers, 20 warps per SM) wins on the whole
-                               job -- config C4 5.37 s against 5.90 s (profiles/r02p_variants.log) */
+                               16 warps per SM) walks one chunk faster, 4 (96 registers, 20 warps per SM) won on the whole
+                               job of config C4 when the two were timed against each other */
 #endif
 #ifndef BR_WALK_G_SMALL
 #define BR_WALK_G_SMALL 1   /* rows fetched together for the 16/32-entry rings */
@@ -656,8 +656,8 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
   k_radix_scatter<8, true><<<ntiles, 256, 0, st>>>(K1, V1, n, hist, ntiles, K2, S, rank);
   k_seg<u16><<<(n + 1 + 255) / 256, 256, 0, st>>>(K2, n, P.nbuckets, seg);
   }
-  // (the 16/32-entry rings of quality 5-6 gain nothing from tags -- measured: C2 58.1 ms with, 56.2 ms without -- so only
-  // the deep rings of quality 7-9 use them: config C4 5.46 s -> 3.36 s)
+  // (the 16/32-entry rings of quality 5-6 gained nothing from tags when timed on C2, so only the deep rings of quality 7-9,
+  // where most of the 256 ring entries are hash collisions whose bytes need not be fetched, use them)
   if (P.block_bits >= 6) k_tags<<<(n + 255) / 256, 256, 0, st>>>(data, S, n, tagS);
   s.tagS = tagS;
   CK(cudaMemsetAsync(bits_latest, 0, nwords * 4, st));

@@ -93,7 +93,7 @@ BR_DEV u32 br_hash_key_v(const BrParams& P, u64 v) {
 }
 #ifndef BR_WALK_SPEC1
 #define BR_WALK_SPEC1 0   /* G == 1: request the candidates' first bytes before their stored bit is known
-                             (measured: 33.2 against 32.7 ms of k_walk per 100 MB of text -- no gain, off) */
+                             (timed on 100 MB of text: no gain, off) */
 #endif
 struct BrWalk {
   const BrStream* s;

@@ -60,8 +60,8 @@ static inline int br_derive_params(int quality, int lgwin, u32 size_hint, u32 n,
   P->step_cap = 4096;
   P->sweep_epoch = 3;    // text / web input settles in 3 launches; what is still dirty then is swept run by run
   P->force_epoch = 64;
-  // pilot launch (BrParams::pilot): pays where a chunk walk is expensive (the deep rings of quality 7-9: config C4 3.37 s ->
-  // 2.75 s, a quarter fewer chunk walks); at quality 5-6 the extra launch costs more than the saved walks (C2 54.4 -> 59.9 ms)
+  // pilot launch (BrParams::pilot): pays where a chunk walk is expensive (the deep rings of quality 7-9: a quarter fewer
+  // chunk walks on config C4); at quality 5-6 the extra launch costs more than the saved walks
   P->pilot = (n >= BR_SMALL_STREAM && P->block_bits >= 6) ? 1u : 0u;
   P->sweep_blocks = P->lgblock >= 21 ? 1u : (1u << (21 - P->lgblock));   // sweeps are at most 2 MiB of input long
   return 1;

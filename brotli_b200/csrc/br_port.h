@@ -1,6 +1,6 @@
 // br_port.h -- thin layer that lets the warp-task device code (br_lz77.h, br_entropy.h)
 // also be compiled by g++ for the CPU "sim" harness under tests/sim/ (test infrastructure,
-// never shipped).  In the product build (nvcc, sm_100a) every BR_DEV function is
+// never shipped).  In the product build (nvcc, sm_90a) every BR_DEV function is
 // __device__-only: there is no host implementation of the hot path in the library.
 //
 // Programming model: "one warp = one task".  Scalar control flow is executed redundantly by

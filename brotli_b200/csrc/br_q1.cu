@@ -174,7 +174,7 @@ struct BrQ1Job {
   Pinned h_in, h_out, h_off;
   u32 log2_n = 0;
   int sm_count = 0;
-  u32 warps_per_sm = 16, first_width = 32;   // tuning knobs (env BR_Q1_WARPS_PER_SM, BR_Q1_FIRST_WIDTH); 16: r02l sweep
+  u32 warps_per_sm = 16, first_width = 32;   // tuning knobs (env BR_Q1_WARPS_PER_SM, BR_Q1_FIRST_WIDTH); 16: best of a sweep of warps per SM
   bool shm_ok = false;        // the device grants k_q1_parse_shm its shared memory
   int kernel_choice = 0;      // 0 / 1 global-memory tables, 2 on-chip tables whenever the fragments fit (env BR_Q1_KERNEL)
   BrQ1Stats stats = {};
@@ -291,10 +291,10 @@ extern "C" int br_q1_compress_batch(BrQ1Job* j, int lgwin, size_t count, const u
   u32 max_frag = 0;
   for (auto& f : frags) if (f.size > max_frag) max_frag = f.size;
   // table and input on chip when every fragment fits (<= 64 KiB) and there are enough of them to fill the SMs
-  // The on-chip variant is bit-exact but measured 4.3x SLOWER on BASELINE config 5 (profiles/r02l_q1_variants.log: parse
-  // 265 ms against 58-61 ms): with the 128 KiB table only ONE warp fits an SM, every instruction latency of its
-  // dependent probe chain is exposed, and 148 latency-bound warps lose to 16-48 warps per SM that hide each other's
-  // HBM round trips.  It stays selectable (BR_Q1_KERNEL=2) for the record; the default is the global-table kernel.
+  // The on-chip variant is bit-exact but slower on BASELINE config 5: with the 128 KiB table only ONE warp fits an SM,
+  // every instruction latency of its dependent probe chain is exposed, and one latency-bound warp per SM loses to 16
+  // warps per SM that hide each other's HBM round trips.  It stays selectable (BR_Q1_KERNEL=2); the default is the
+  // global-table kernel.
   const bool on_chip = j->shm_ok && max_frag <= 65536u && j->kernel_choice == 2;
   if (nfr) {
     if (on_chip) {

@@ -4,7 +4,7 @@
 // :228, StoreCommands :458, BuildAndStoreCommandPrefixCode :58, ShouldCompress :526) driven by
 // c/enc/encode.c:1425 BrotliEncoderCompressStreamFast.  Every fragment (one call of :612: at most
 // 1 << lgwin bytes, fresh zeroed hash table) is independent of every other one; inside a fragment
-// the 128 KiB blocks share the table.  The B200 shape:
+// the 128 KiB blocks share the table.  The GPU shape:
 //
 //   parse   one WARP per fragment (k_q1_parse).  The reference's trawl loop visits a predictable
 //           sequence of positions until a match turns up (skip heuristic :262), so the 32 lanes

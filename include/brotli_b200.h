@@ -7,7 +7,7 @@
  * (go/cbrotli/writer.go:30) and the JNI wrapper (java/org/brotli/wrapper/enc/encoder_jni.cc:78)
  * can link against this library instead of libbrotlienc.  See INTEGRATION.md.
  *
- * The hot path runs on an NVIDIA B200 (sm_100a).  There is NO CPU implementation inside
+ * The hot path runs on an NVIDIA H100 (sm_90a).  There is NO CPU implementation inside
  * the library: without a CUDA device, or for parameters outside the implemented path
  * (quality 1..9, no custom dictionary, modes GENERIC/TEXT: limits below), the entry points
  * return BROTLI_FALSE / NULL instead of producing different bytes.
@@ -37,7 +37,7 @@ extern "C" {
 
 #define BROTLI_B200_API BROTLI_ENC_API
 
-/* ---- B200 extensions (not in the reference API) ------------------------------------ */
+/* ---- device-resident extensions (not in the reference API) ------------------------ */
 /* Same as BrotliEncoderCompress but input and output live in DEVICE memory of the current
  * CUDA device (plain device pointers).  *encoded_size: in = capacity, out = bytes written. */
 BROTLI_B200_API BROTLI_BOOL BrotliB200CompressDevice(int quality, int lgwin, size_t input_size, const void* d_input, size_t* encoded_size, void* d_encoded);

@@ -1,6 +1,8 @@
 """ctypes loaders for the checker libraries (oracle/ and oracle/_ref) and the product
 C-ABI (brotli_b200/libbrotlienc_b200.so).  Test infrastructure only."""
 import ctypes as C
+import hashlib
+import json
 import os
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -9,6 +11,7 @@ PROBE_SO = os.path.join(ROOT, "oracle", "_ref", "libbrotli_probe.so")
 ORACLE_SO = os.path.join(ROOT, "oracle", "liboracle.so")
 TABLES = os.path.join(ROOT, "brotli_b200", "data", "brotli_tables.bin")
 PRODUCT_SO = os.path.join(ROOT, "brotli_b200", "libbrotlienc_b200.so")
+REF_CALLS = os.path.join(ROOT, "tests", "golden", "reference_calls.json")
 
 _u8p = C.POINTER(C.c_uint8)
 
@@ -32,7 +35,7 @@ def zeroed_malloc():
 
 
 class Ref:
-    """The unmodified reference compiled from /root/reference (oracle/Makefile)."""
+    """The unmodified reference encoder, live (oracle/_ref, built by oracle/Makefile from a google/brotli tree)."""
 
     def __init__(self, path=REF_SO):
         self.lib = C.CDLL(path, mode=os.RTLD_LOCAL)
@@ -107,6 +110,8 @@ def ref_compress_stream(ref, data, quality, lgwin, chunk, out_buf=1 << 19):
     """Drives the reference's streaming API the way c/tools/brotli.c:1357 does: PROCESS calls of
     `chunk` bytes, FINISH once the input is exhausted (an extra empty call when the size is a
     multiple of `chunk`, like feof() after a full read)."""
+    if isinstance(ref, RecordedRef):
+        return ref.compress_stream(data, quality, lgwin, chunk, out_buf)
     L = ref.lib
     L.BrotliEncoderCreateInstance.restype = C.c_void_p
     L.BrotliEncoderCreateInstance.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
@@ -146,6 +151,8 @@ def ref_compress_stream(ref, data, quality, lgwin, chunk, out_buf=1 << 19):
 def ref_stream_ops(ref, data, quality, lgwin, sizes, ops, out_buf=1 << 16, params=None):
     """Drives the reference's CompressStream with an explicit list of (size, op) calls, draining the
     output after each call the way encode.h:473 asks (repeat until no input and no more output)."""
+    if isinstance(ref, RecordedRef):
+        return ref.stream_ops(data, quality, lgwin, sizes, ops, out_buf, params)
     L = ref.lib
     L.BrotliEncoderCreateInstance.restype = C.c_void_p
     L.BrotliEncoderCreateInstance.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
@@ -175,3 +182,89 @@ def ref_stream_ops(ref, data, quality, lgwin, sizes, ops, out_buf=1 << 16, param
                 break
     L.BrotliEncoderDestroyInstance(s)
     return bytes(out)
+
+
+class Digest(object):
+    """A byte string of the reference kept as its length and the first 128 bits of its SHA-256; compares equal to the
+    bytes it was made from."""
+
+    def __init__(self, n, sha):
+        self.n, self.sha = n, sha
+
+    def __eq__(self, other):
+        if isinstance(other, Digest):
+            return (self.n, self.sha) == (other.n, other.sha)
+        if isinstance(other, (bytes, bytearray)):
+            return len(other) == self.n and hashlib.sha256(other).hexdigest()[:32] == self.sha
+        return NotImplemented
+
+    def __ne__(self, other):
+        r = self.__eq__(other)
+        return r if r is NotImplemented else not r
+
+    __hash__ = None
+
+    def __len__(self):
+        return self.n
+
+    def __repr__(self):
+        return "Digest(%d bytes, sha256 %s)" % (self.n, self.sha[:16])
+
+
+def _digest(b):
+    return [len(b), hashlib.sha256(b).hexdigest()[:32]]
+
+
+def _tag(b):
+    return "%d:%s" % (len(b), (b.sha if isinstance(b, Digest) else hashlib.sha256(b).hexdigest())[:24])
+
+
+_CALLS = None
+
+
+class RecordedRef(object):
+    """The unmodified reference encoder and decoder as the tests compare against them: every result the tests ask for was
+    computed once by the compiled reference (oracle/_ref) and is replayed from tests/golden/reference_calls.json as a
+    Digest, so the comparisons run where the reference is not available.  A call that was not recorded -- above all a
+    decompress() of bytes the reference did not produce -- fails.  With BROTLI_REF_RECORD=<file> (and oracle/_ref
+    built) every call runs the live reference instead and appends its result to <file> as a JSON line;
+    tests/golden/merge_reference_calls.py folds such files into reference_calls.json."""
+
+    def __init__(self):
+        global _CALLS
+        self.record = os.environ.get("BROTLI_REF_RECORD")
+        self.live = Ref() if self.record else None
+        if _CALLS is None:
+            _CALLS = json.load(open(REF_CALLS)) if os.path.exists(REF_CALLS) else {}
+
+    def _call(self, key, run):
+        if self.live is not None:
+            v = run(self.live)
+            val = v if isinstance(v, int) else _digest(v)
+            with open(self.record, "a") as f:
+                f.write(json.dumps({"key": key, "value": val}) + "\n")
+            return v
+        if key not in _CALLS:
+            raise AssertionError("no recorded reference result for %r: the reference was never asked this (for decompress: "
+                                 "the bytes are not what the reference encoder produced)" % key)
+        val = _CALLS[key]
+        return val if isinstance(val, int) else Digest(*val)
+
+    def compress(self, data, quality, lgwin, mode=0):
+        return self._call("compress q%d w%d m%d %s" % (quality, lgwin, mode, _tag(data)),
+                          lambda r: r.compress(data, quality, lgwin, mode))
+
+    def decompress(self, comp, max_out):
+        return self._call("decompress %d %s" % (max_out, _tag(comp)), lambda r: r.decompress(comp, max_out))
+
+    def max_compressed_size(self, n):
+        return self._call("max_compressed_size %d" % n, lambda r: int(r.lib.BrotliEncoderMaxCompressedSize(n)))
+
+    def compress_stream(self, data, quality, lgwin, chunk, out_buf):
+        return self._call("compress_stream q%d w%d chunk%d %s" % (quality, lgwin, chunk, _tag(data)),
+                          lambda r: ref_compress_stream(r, data, quality, lgwin, chunk, out_buf))
+
+    def stream_ops(self, data, quality, lgwin, sizes, ops, out_buf, params):
+        prm = sorted((params or {}).items())
+        return self._call("stream_ops q%d w%d sizes%s ops%s params%s %s" % (quality, lgwin, list(sizes), list(ops), prm, _tag(data)),
+                          lambda r: ref_stream_ops(r, data, quality, lgwin, sizes, ops, out_buf, params))

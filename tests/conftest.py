@@ -8,7 +8,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # The reference is not deterministic on a dirty heap for some FLUSH sequences (brotli_libs.zeroed_malloc): the CPU suite,
     # whose randomized sim tests can meet such a sequence, runs with zeroed malloc.  The GPU suite (-m gpu) keeps the allocator
     # as it is: none of its call sequences runs a block across the ring's end in the first lap behind a short first write, and

@@ -24,7 +24,7 @@ ENCODE_H = os.path.join(ROOT, "include", "brotli", "encode.h")
 
 
 def declared_symbols():
-    """Every function the public headers declare: the reference API (include/brotli/encode.h) and the B200 extensions."""
+    """Every function the public headers declare: the reference API (include/brotli/encode.h) and the device-resident extensions."""
     names = set()
     for path, macro in ((HEADER, "BROTLI_B200_API"), (ENCODE_H, "BROTLI_ENC_API")):
         names |= set(re.findall(macro + r"[^;(]*?\b(Brotli\w+)\s*\(", open(path).read()))

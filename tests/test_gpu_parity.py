@@ -1,5 +1,5 @@
 """GPU suite (-m gpu): the CUDA path, called through the C ABI, against the golden vectors of the
-compiled reference, the oracle, and -- where it travelled -- oracle/_ref itself.  Bit-exact."""
+compiled reference, the oracle, and the reference's recorded results for the same calls (brotli_libs.RecordedRef).  Bit-exact."""
 import ctypes as C
 import hashlib
 import json
@@ -8,7 +8,7 @@ import os
 import numpy as np
 import pytest
 
-from brotli_libs import REF_SO, Oracle, Ref, ref_compress_stream, ref_stream_ops
+from brotli_libs import Oracle, RecordedRef, ref_compress_stream, ref_stream_ops
 from golden_cases import make_case
 
 pytestmark = pytest.mark.gpu
@@ -96,13 +96,12 @@ def _drive(b200, d, q, w, sizes, ops):
     return out
 
 
-@pytest.mark.skipif(not os.path.exists(REF_SO), reason="oracle/_ref did not travel")
 def test_streaming_flush_and_metadata(b200):
     """FLUSH and EMIT_METADATA at quality 5..9 (encode.c:1356, :1549): byte-identical to the reference's CompressStream for
     the same call sequence -- flushes inside and at block boundaries, a flush / metadata before any input, metadata between
     data, repeated operations at one position, FINISH without input behind a full block, and everything flushed bytewise."""
     from corpus import synth_binary, synth_text
-    ref = Ref()
+    ref = RecordedRef()
     for d in (synth_text(700000, 61), synth_binary(900000, 62)):
         n = len(d)
         for q, w in ((5, 22), (9, 24), (6, 18)):
@@ -132,12 +131,11 @@ def test_streaming_flush_and_metadata(b200):
     assert ref.decompress(part + rest, len(d)) == d
 
 
-@pytest.mark.skipif(not os.path.exists(REF_SO), reason="oracle/_ref did not travel")
 def test_lgblock_and_context_modeling_parameters(b200):
     """BROTLI_PARAM_LGBLOCK (encode.h:184, quality.h:76) and BROTLI_PARAM_DISABLE_LITERAL_CONTEXT_MODELING (encode.h:191,
     encode.c:561) through the streaming API, against the reference with the same parameters."""
     from corpus import synth_web
-    ref = Ref()
+    ref = RecordedRef()
     L = b200.lib()
     d = synth_web(1500000, 65)
     for q, w in ((5, 22), (9, 24)):
@@ -155,13 +153,12 @@ def test_lgblock_and_context_modeling_parameters(b200):
             assert got == want, (q, w, lgb, dis)
 
 
-@pytest.mark.skipif(not os.path.exists(REF_SO), reason="oracle/_ref did not travel")
 def test_stream_offset_stitches_shards(b200):
     """SURVEY.md 8e: one valid stream out of independently compressed shards -- every shard but the first is compressed with
     BROTLI_PARAM_STREAM_OFFSET = its start (encode.h:231), every shard but the last ends with FLUSH instead of FINISH.
     Each shard equals the reference run with the same parameters and calls; the concatenation decodes to the input."""
     from corpus import synth_web
-    ref = Ref()
+    ref = RecordedRef()
     L = b200.lib()
     d = synth_web(1800000, 68)
     cuts = [0, 500000, 1300001, len(d)]
@@ -283,19 +280,17 @@ def test_batch_of_small_streams(b200):
         assert got[k] == ora.compress(x, 5, 22), k
 
 
-@pytest.mark.skipif(not os.path.exists(REF_SO), reason="oracle/_ref did not travel")
 def test_full_size_properties(b200):
     """BASELINE.json's full size (100 MB, q5, lgwin 22): equality with the reference run on the
     box's CPU, and the size-independent property decode(encode(x)) == x via the reference decoder."""
     from corpus import synth_text
-    ref = Ref()
+    ref = RecordedRef()
     d = synth_text(100_000_000)
     out = b200.compress_oneshot(d, 5, 22)
     assert ref.decompress(out, len(d)) == d
     assert out == ref.compress(d, 5, 22)
 
 
-@pytest.mark.skipif(not os.path.exists(REF_SO), reason="oracle/_ref did not travel")
 def test_q9_ring_wrap_and_nonsettling_inputs(b200):
     """Quality 9 / lgwin 24 beyond the 32 MiB ring buffer of the reference (BASELINE config C4's path: H6, 256-entry
     rings, 256 KiB input blocks), on the Silesia-shaped binary mix, and inputs whose parse never settles by itself --
@@ -303,7 +298,7 @@ def test_q9_ring_wrap_and_nonsettling_inputs(b200):
     encoder must never fail (encode.c:1340-1353) and must equal the reference run on the box."""
     import numpy as np
     from corpus import synth_binary
-    ref = Ref()
+    ref = RecordedRef()
     cases = [("binary mix 48 MiB", synth_binary(48 << 20, 91), 9, 24),
              ("uniform noise 24 MiB", np.random.RandomState(92).randint(0, 256, 24 << 20, dtype=np.uint8).tobytes(), 9, 24),
              ("uniform noise 16 MiB q5", np.random.RandomState(93).randint(0, 256, 16 << 20, dtype=np.uint8).tobytes(), 5, 22),
@@ -313,12 +308,11 @@ def test_q9_ring_wrap_and_nonsettling_inputs(b200):
         assert out == ref.compress(d, q, w), name
 
 
-@pytest.mark.skipif(not os.path.exists(REF_SO), reason="oracle/_ref did not travel")
 def test_config3_slice_and_config5_streams(b200):
     """BASELINE config C3 (web mix, quality 5, lgwin 22) on a 256 MiB slice, and config C5 on 1000 of its 64 KiB streams
     (quality 1, one device batch), each against the reference run on the box."""
     from corpus import synth_web
-    ref = Ref()
+    ref = RecordedRef()
     web = synth_web(256 << 20)
     out = b200.compress_oneshot(web, 5, 22)
     assert out == ref.compress(web, 5, 22)
@@ -365,13 +359,12 @@ def test_cli_dropin_stdin(b200, tmp_path):
         assert outs[0] == outs[1] and len(outs[0]) > 0, (n, q, w)
 
 
-@pytest.mark.skipif(not os.path.exists(REF_SO), reason="oracle/_ref did not travel")
 def test_one_shot_wrapper_rules(b200):
     """encode.c:1296-1353 / quality.h:60: quality 1 with lgwin above 24 is sanitised to 24 (no large window at quality <= 2);
     an output buffer that is too small fails; an incompressible input still fits BrotliEncoderMaxCompressedSize."""
     import numpy as np
     from corpus import synth_text
-    ref = Ref()
+    ref = RecordedRef()
     L = b200.lib()
     d = synth_text(200000, 66)
     assert b200.compress_oneshot(d, 1, 27) == ref.compress(d, 1, 27) == ref.compress(d, 1, 24)
@@ -431,15 +424,14 @@ def test_q1_streaming_call_pattern(b200):
         out += c.finish()
         calls = [a for a in sizes if a] + [0]
         assert out == ora.compress_q1_stream(d, 22, calls), sizes
-    if os.path.exists(REF_SO):
-        ref = Ref()
-        c = b200.Compressor(quality=1, lgwin=18)
-        out = b""
-        for o in range(0, len(d), 1 << 19):
-            out += c.process(d[o:o + (1 << 19)])
-        out += c.finish()
-        assert out == ref_compress_stream(ref, d, 1, 18, 1 << 19)
-        assert ref.decompress(out, len(d)) == d
+    ref = RecordedRef()
+    c = b200.Compressor(quality=1, lgwin=18)
+    out = b""
+    for o in range(0, len(d), 1 << 19):
+        out += c.process(d[o:o + (1 << 19)])
+    out += c.finish()
+    assert out == ref_compress_stream(ref, d, 1, 18, 1 << 19)
+    assert ref.decompress(out, len(d)) == d
 
 
 def test_q1_cli_dropin(b200, tmp_path):
@@ -482,11 +474,9 @@ def test_q1_flush(b200):
                 else:
                     out += c._stream(piece, c._FINISH)
             assert out == ora.compress_q1_stream(d, w, sizes, ops), (sizes, ops, w)
-            if os.path.exists(REF_SO):
-                assert out == ref_stream_ops(Ref(), d, 1, w, sizes, ops)
+            assert out == ref_stream_ops(RecordedRef(), d, 1, w, sizes, ops)
 
 
-@pytest.mark.skipif(not os.path.exists(REF_SO), reason="oracle/_ref did not travel")
 def test_q1_stream_beyond_one_device_segment(b200):
     """Quality 1 has no stream-size limit: input above one device segment (128 MiB) runs as several, a segment that
     neither flushes nor finishes ends mid-byte and the next starts behind its pending bits (br_api.cc q1_run).
@@ -499,7 +489,7 @@ def test_q1_stream_beyond_one_device_segment(b200):
     d[idx] = rng.integers(0, 256, idx.size, dtype=np.uint8)
     d[(1 << 27) - 3_000_000:(1 << 27) + 3_000_000] = rng.integers(0, 256, 6_000_000, dtype=np.uint8)   # raw fragments across a cut
     d = d.tobytes()
-    ref = Ref()
+    ref = RecordedRef()
     for w in (22, 18):
         assert b200.compress_oneshot(d, 1, w) == ref.compress(d, 1, w), w
     step = (24 << 20) + 1

@@ -196,12 +196,10 @@ def _sim_cuts(sim, d, q, w, hint, cuts, kinds, is_final, finish_empty=0, lgblock
 def test_sim_flush_cuts_and_parameters(sim):
     """The device code with the input cut by FLUSH operations (encode.c:1356, :1700), with FINISH arriving without input
     behind a full block (encode.c:520), and with BROTLI_PARAM_LGBLOCK / DISABLE_LITERAL_CONTEXT_MODELING, against the
-    reference's CompressStream driven with the same calls (needs oracle/_ref)."""
-    from brotli_libs import REF_SO, Ref, ref_stream_ops
-    if not os.path.exists(REF_SO):
-        pytest.skip("oracle/_ref not built")
+    reference's CompressStream driven with the same calls."""
+    from brotli_libs import RecordedRef, ref_stream_ops
     from corpus import synth_binary, synth_text, synth_web
-    ref = Ref()
+    ref = RecordedRef()
     for d in (synth_text(400000, 3), synth_binary(600000, 5)):
         n = len(d)
         for q, w in ((5, 22), (9, 24), (7, 19)):
@@ -379,11 +377,9 @@ def test_sim_stream_offset(sim):
     """BROTLI_PARAM_STREAM_OFFSET (encode.h:231, the sanctioned way to stitch shards into one stream, SURVEY.md 8e): no
     window bits, poisoned distance cache (encode.c:656), dictionary distances counted from the virtual start
     (backward_references_inc.h:94), and the first two bytes flushed on their own (encode.c:1704) -- against the reference."""
-    from brotli_libs import REF_SO, Ref, ref_stream_ops
-    if not os.path.exists(REF_SO):
-        pytest.skip("oracle/_ref not built")
+    from brotli_libs import RecordedRef, ref_stream_ops
     from corpus import synth_text, synth_web
-    ref = Ref()
+    ref = RecordedRef()
     for d in (synth_text(300000, 4), synth_web(500000, 10)):
         for q, w in ((5, 22), (9, 24), (6, 18)):
             for off in (1, 1000, 1 << 20, 1 << 30):
@@ -443,11 +439,9 @@ def test_sim_q234_flush_cuts(sim):
     """Qualities 2..4 with the input cut by FLUSH operations, against the reference's CompressStream driven with the same
     calls: input blocks of 1 << 14 bytes below quality 4 (quality.h:81), the MAX_NUM_DELAYED_SYMBOLS flush rule
     (encode.c:1152), FINISH without input behind a full block."""
-    from brotli_libs import REF_SO, Ref, ref_stream_ops
-    if not os.path.exists(REF_SO):
-        pytest.skip("oracle/_ref not built")
+    from brotli_libs import RecordedRef, ref_stream_ops
     from corpus import synth_binary, synth_text
-    ref = Ref()
+    ref = RecordedRef()
     for d in (synth_text(300000, 3), synth_binary(400000, 5)):
         n = len(d)
         for q, w in ((2, 22), (3, 18), (4, 22), (4, 12)):
@@ -568,11 +562,9 @@ def test_sim_flush_just_behind_a_block_boundary(sim):
     (hash_longest_match_quickly_inc.h:119 / hash_longest_match64_inc.h:127: num_bytes >= HashTypeLength - 1); the block behind
     it stitches instead, and its three positions reach back across the short block into the block in front.  Their owner must
     still commit them (br_commit_bits; found by a randomized FLUSH campaign: q3, lgwin 12, flush at 14 * 16384 + 2)."""
-    from brotli_libs import REF_SO, Ref, ref_stream_ops
-    if not os.path.exists(REF_SO):
-        pytest.skip("oracle/_ref not built")
+    from brotli_libs import RecordedRef, ref_stream_ops
     from corpus import synth_text
-    ref = Ref()
+    ref = RecordedRef()
     d = synth_text(200000, 77)
     n = len(d)
     for q, w in ((3, 12), (2, 22), (4, 16), (5, 22), (7, 17)):
