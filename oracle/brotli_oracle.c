@@ -51,6 +51,39 @@ static double fast_log2(size_t v) {
 }
 double oracle_fast_log2(size_t v) { return fast_log2(v); }
 
+/* Edge counters: how often the entropy stage took the branches that ordinary data rarely reaches, so that a test
+ * can prove its input still reaches the branch it was built for (tests/entropy_cases.py).  They only count; the
+ * output never depends on them.  A metablock replaced by a raw one (encode.c:604) leaves them as they were.
+ *   retry_*: count_limit doublings in BrotliCreateHuffmanTree for symbol trees (depth 15; told apart by alphabet
+ *       size: 256 literals, 704 commands, 64 / 140 distances, other: block switches and context maps) and the
+ *       code-length code (retry_cl, depth 5), and in BrotliBuildAndStoreHuffmanTreeFast (retry_fast, depth 14)
+ *   simple_nsym1..4, simple_select0/1: codes stored as simple prefix codes by NSYM; for NSYM 4 the tree-select bit
+ *   rle_lt16 / rle_lt28 / rle_full: exits of BrotliOptimizeHuffmanCountsForRle (its nonzeros < 5 exit cannot be
+ *       taken behind the first one); rle_holes: counts filled
+ *   reps7 / reps11: the reps == 7 (non-zero) and reps == 11 (zero) special cases of the code-length run writers
+ *   rle_use_nz / rle_use_z: DecideOverRleUse chose runs for a tree of more than 50 symbols
+ *   ctx_nc1/2/3/13: compressed metablocks (quality 4+) by literal context count; lit_cap_nc*: those whose literal
+ *       split reached the 256 / nc type cap; split_back: blocks merged into the type before last (action 2)
+ *   max_lit_types / max_lit_trees / max_cmd_types / max_dist_types: per metablock
+ *   max_insert / max_copy / max_block_len / max_distance: the longest emitted (distance: explicit codes only) */
+#define EDGE_FIELDS(X) X(retry_lit) X(retry_cmd) X(retry_dist) X(retry_other) X(retry_cl) X(retry_fast) \
+  X(simple_nsym1) X(simple_nsym2) X(simple_nsym3) X(simple_nsym4) X(simple_select0) X(simple_select1) X(rle_lt16) X(rle_lt28) X(rle_full) X(rle_holes) \
+  X(reps7) X(reps11) X(rle_use_nz) X(rle_use_z) X(ctx_nc1) X(ctx_nc2) X(ctx_nc3) X(ctx_nc13) X(lit_cap_nc1) \
+  X(lit_cap_nc2) X(lit_cap_nc3) X(lit_cap_nc13) X(split_back) X(max_lit_types) X(max_lit_trees) X(max_cmd_types) \
+  X(max_dist_types) X(max_insert) X(max_copy) X(max_block_len) X(max_distance)
+#define EDGE_MEMBER(f) uint64_t f;
+#define EDGE_NAME(f) #f ","
+static struct { EDGE_FIELDS(EDGE_MEMBER) } g_edge;
+#define EDGE_MAX(f, v) do { if ((uint64_t)(v) > g_edge.f) g_edge.f = (uint64_t)(v); } while (0)
+void oracle_edge_stats_reset(void) { memset(&g_edge, 0, sizeof(g_edge)); }
+/* The counters as uint64 words in the order of oracle_edge_stats_names(); returns how many there are. */
+size_t oracle_edge_stats(uint64_t* out, size_t cap) {
+  const size_t n = sizeof(g_edge) / sizeof(uint64_t);
+  if (out) memcpy(out, &g_edge, (cap < n ? cap : n) * sizeof(uint64_t));
+  return n;
+}
+const char* oracle_edge_stats_names(void) { return EDGE_FIELDS(EDGE_NAME); }
+
 int oracle_init(const uint8_t* blob, size_t len) {
   const uint8_t* p;
   if (len != 8 + 32 + 128 + 122784 + 65536 + 32768 + 2048) return 0;
@@ -660,6 +693,11 @@ static void create_huffman_tree(const uint32_t* data, size_t length, int tree_li
         tree[j_end + 1] = sentinel; }
     }
     if (set_depth((int)(2 * n - 1), tree, depth, tree_limit)) break;
+    if (tree_limit == 5) ++g_edge.retry_cl;
+    else if (length == 256) ++g_edge.retry_lit;
+    else if (length == 704) ++g_edge.retry_cmd;
+    else if (length == 64 || length == 140) ++g_edge.retry_dist;
+    else ++g_edge.retry_other;
   }
 }
 /* entropy_encode.c:474 BrotliConvertBitDepthsToSymbols */
@@ -683,7 +721,7 @@ static void optimize_counts_for_rle(size_t length, uint32_t* counts, uint8_t* go
   size_t nonzero_count = 0, stride, limit, sum, i;
   const size_t streak_limit = 1240;
   for (i = 0; i < length; i++) if (counts[i]) ++nonzero_count;
-  if (nonzero_count < 16) return;
+  if (nonzero_count < 16) { ++g_edge.rle_lt16; return; }
   while (length != 0 && counts[length - 1] == 0) --length;
   if (length == 0) return;
   {
@@ -695,10 +733,11 @@ static void optimize_counts_for_rle(size_t length, uint32_t* counts, uint8_t* go
       size_t zeros = length - nonzeros;
       if (zeros < 6)
         for (i = 1; i < length - 1; ++i)
-          if (counts[i - 1] != 0 && counts[i] == 0 && counts[i + 1] != 0) counts[i] = 1;
+          if (counts[i - 1] != 0 && counts[i] == 0 && counts[i + 1] != 0) { counts[i] = 1; ++g_edge.rle_holes; }
     }
-    if (nonzeros < 28) return;
+    if (nonzeros < 28) { ++g_edge.rle_lt28; return; }
   }
+  ++g_edge.rle_full;
   memset(good_for_rle, 0, length);
   {
     uint32_t symbol = counts[0]; size_t step = 0;
@@ -745,7 +784,7 @@ static void rev(uint8_t* v, size_t s, size_t e) {
 static void write_reps(uint8_t prev, uint8_t value, size_t reps, size_t* ts,
                        uint8_t* tree, uint8_t* extra) {
   if (prev != value) { tree[*ts] = value; extra[*ts] = 0; ++(*ts); --reps; }
-  if (reps == 7) { tree[*ts] = value; extra[*ts] = 0; ++(*ts); --reps; }
+  if (reps == 7) { tree[*ts] = value; extra[*ts] = 0; ++(*ts); --reps; ++g_edge.reps7; }
   if (reps < 3) {
     size_t i; for (i = 0; i < reps; ++i) { tree[*ts] = value; extra[*ts] = 0; ++(*ts); }
   } else {
@@ -761,7 +800,7 @@ static void write_reps(uint8_t prev, uint8_t value, size_t reps, size_t* ts,
   }
 }
 static void write_reps_zeros(size_t reps, size_t* ts, uint8_t* tree, uint8_t* extra) {
-  if (reps == 11) { tree[*ts] = 0; extra[*ts] = 0; ++(*ts); --reps; }
+  if (reps == 11) { tree[*ts] = 0; extra[*ts] = 0; ++(*ts); --reps; ++g_edge.reps11; }
   if (reps < 3) {
     size_t i; for (i = 0; i < reps; ++i) { tree[*ts] = 0; extra[*ts] = 0; ++(*ts); }
   } else {
@@ -791,6 +830,7 @@ static void write_huffman_tree(const uint8_t* depth, size_t length, size_t* ts,
       i += reps;
     }
     rle_nz = tnz > cnz * 2; rle_z = tz > cz * 2;
+    g_edge.rle_use_nz += rle_nz; g_edge.rle_use_z += rle_z;
   }
   for (i = 0; i < new_length;) {
     uint8_t v = depth[i]; size_t reps = 1;
@@ -853,6 +893,9 @@ static void store_simple_tree(const uint8_t* depths, size_t* symbols, size_t num
       if (depths[symbols[j]] < depths[symbols[i]]) { size_t t = symbols[j]; symbols[j] = symbols[i]; symbols[i] = t; }
   for (i = 0; i < num; ++i) wbits(w, max_bits, symbols[i]);
   if (num == 4) wbits(w, 1, depths[symbols[0]] == 1 ? 1 : 0);
+  if (num == 2) ++g_edge.simple_nsym2;
+  else if (num == 3) ++g_edge.simple_nsym3;
+  else { ++g_edge.simple_nsym4; if (depths[symbols[0]] == 1) ++g_edge.simple_select1; else ++g_edge.simple_select0; }
 }
 /* brotli_bit_stream.c:349 BuildAndStoreHuffmanTree */
 static void build_and_store_tree(const uint32_t* histo, size_t histo_len, size_t alphabet_size,
@@ -869,6 +912,7 @@ static void build_and_store_tree(const uint32_t* histo, size_t histo_len, size_t
     wbits(w, 4, 1);
     wbits(w, max_bits, s4[0]);
     depth[s4[0]] = 0; bits[s4[0]] = 0;
+    ++g_edge.simple_nsym1;
     return;
   }
   memset(depth, 0, histo_len);
@@ -1004,6 +1048,7 @@ static void splitter_finish_block(Splitter* s, int is_final) {
       }
       ++s->num_blocks;
       s->block_size = 0; s->merge_last_count = 0; s->target_block_size = s->min_block_size;
+      ++g_edge.split_back;
     } else {
       split->lengths[s->num_blocks - 1] += (uint32_t)s->block_size;
       for (i = 0; i < nc; ++i) {
@@ -1270,6 +1315,15 @@ static void encode_context_map(const uint32_t* cmap, size_t cmap_size, size_t nu
   free(rle);
 }
 
+static void edge_cmd(const Cmd* c, int lgwin) {
+  const uint32_t dcode = cmd_restore_dcode(c);
+  EDGE_MAX(max_insert, c->insert_len);
+  EDGE_MAX(max_copy, cmd_copy_len(c));
+  /* backward references only: a static-dictionary word lies beyond max_backward (encode.c:1240) */
+  if (cmd_copy_len(c) && c->cmd_prefix >= 128 && dcode >= 16 && dcode - 15 <= ((1u << lgwin) - 16))
+    EDGE_MAX(max_distance, dcode - 15);
+}
+
 /* brotli_bit_stream.c:82 StoreCommandExtra */
 static void store_cmd_extra(const Cmd* c, BitW* w) {
   uint32_t clc = cmd_copy_len_code(c);
@@ -1326,6 +1380,17 @@ static void store_compressed_metablock(Enc* e, size_t start_pos, size_t length,
     for (i = 0; i < lit_split.num_types; ++i)
       for (j = 0; j < 64; ++j) lit_cmap[(i << 6) + j] = (uint32_t)(i * nctx) + smap[j];
   }
+  if (nctx == 1) ++g_edge.ctx_nc1; else if (nctx == 2) ++g_edge.ctx_nc2; else if (nctx == 3) ++g_edge.ctx_nc3; else ++g_edge.ctx_nc13;
+  if (lit_split.num_types == 256 / nctx) {
+    if (nctx == 1) ++g_edge.lit_cap_nc1; else if (nctx == 2) ++g_edge.lit_cap_nc2; else if (nctx == 3) ++g_edge.lit_cap_nc3;
+    else ++g_edge.lit_cap_nc13;
+  }
+  EDGE_MAX(max_lit_types, lit_split.num_types); EDGE_MAX(max_lit_trees, ls.histograms_size);
+  EDGE_MAX(max_cmd_types, cmd_split.num_types); EDGE_MAX(max_dist_types, dist_split.num_types);
+  { const Split* sp[3] = {&lit_split, &cmd_split, &dist_split}; size_t k;   /* lengths are stored with 2+ types only */
+    for (k = 0; k < 3; ++k)
+      if (sp[k]->num_types > 1)
+        for (i = 0; i < sp[k]->num_blocks; ++i) EDGE_MAX(max_block_len, sp[k]->lengths[i]); }
   for (i = 0; i < ls.histograms_size; ++i) optimize_counts_for_rle(256, ls.histograms + i * 256, good_for_rle);
   for (i = 0; i < cs.histograms_size; ++i) optimize_counts_for_rle(704, cs.histograms + i * 704, good_for_rle);
   for (i = 0; i < ds.histograms_size; ++i) optimize_counts_for_rle(64, ds.histograms + i * 64, good_for_rle);
@@ -1362,6 +1427,7 @@ static void store_compressed_metablock(Enc* e, size_t start_pos, size_t length,
   pos = start_pos; p1 = e->prev_byte; p2 = e->prev_byte2;
   for (i = 0; i < ncmd; ++i) {
     const Cmd c = cmds[i]; size_t j;
+    edge_cmd(&c, e->lgwin);
     store_symbol(&ce, c.cmd_prefix, w);
     store_cmd_extra(&c, w);
     if (lit_cmap_size == 0) {
@@ -1410,9 +1476,13 @@ static void write_metablock(Enc* e, size_t end_pos, int is_last) {
     memcpy(e->dist_cache, e->saved_dist_cache, 4 * sizeof(int));
     store_uncompressed(is_last, e->data, e->last_flush_pos, bytes, &w);
   } else {
+    const size_t edge_words = sizeof(g_edge) / sizeof(uint64_t);
+    uint64_t edge_before[sizeof(g_edge) / sizeof(uint64_t)];
+    oracle_edge_stats(edge_before, edge_words);
     if (e->quality < 4) store_metablock_fast_trivial(e, e->last_flush_pos, bytes, is_last, &w);   /* encode.c:543-556 */
     else store_compressed_metablock(e, e->last_flush_pos, bytes, is_last, &w);
     if (bytes + 4 < (w.ix >> 3)) {
+      memcpy(&g_edge, edge_before, sizeof(g_edge));
       memcpy(e->dist_cache, e->saved_dist_cache, 4 * sizeof(int));
       memset(storage, 0, 2 * bytes + 503 + 16);
       storage[0] = e->carry; w.ix = e->carry_bits;
@@ -1582,6 +1652,7 @@ static void store_metablock_fast_trivial(Enc* e, size_t start_pos, size_t length
   pos = start_pos;
   for (i = 0; i < ncmd; ++i) {          /* :1159 StoreDataWithHuffmanCodes */
     const Cmd c = cmds[i]; size_t j;
+    edge_cmd(&c, e->lgwin);
     wbits(w, cmd_depth[c.cmd_prefix], cmd_bits[c.cmd_prefix]);
     store_cmd_extra(&c, w);
     for (j = c.insert_len; j != 0; --j) { wbits(w, lit_depth[in[pos]], lit_bits[in[pos]]); ++pos; }

@@ -216,6 +216,7 @@ static void q1_build_and_store_tree_fast(const uint32_t* histo, size_t total, si
   if (count <= 1) {
     wbits(w, 4, 1); wbits(w, max_bits, symbols[0]);
     depth[symbols[0]] = 0; bits[symbols[0]] = 0;
+    ++g_edge.simple_nsym1;
     return;
   }
   memset(depth, 0, length);
@@ -240,6 +241,7 @@ static void q1_build_and_store_tree_fast(const uint32_t* histo, size_t total, si
         tree[parent + 1] = sentinel;
       }
       if (set_depth((int)(2 * n - 1), tree, depth, 14)) break;
+      ++g_edge.retry_fast;
     }
   }
   depths_to_symbols(depth, length, bits);
@@ -251,6 +253,9 @@ static void q1_build_and_store_tree_fast(const uint32_t* histo, size_t total, si
         if (depth[symbols[j]] < depth[symbols[i]]) { size_t t = symbols[j]; symbols[j] = symbols[i]; symbols[i] = t; }
     for (i = 0; i < count; ++i) wbits(w, max_bits, symbols[i]);
     if (count == 4) wbits(w, 1, depth[symbols[0]] == 1 ? 1 : 0);
+    if (count == 2) ++g_edge.simple_nsym2;
+    else if (count == 3) ++g_edge.simple_nsym3;
+    else { ++g_edge.simple_nsym4; if (depth[symbols[0]] == 1) ++g_edge.simple_select1; else ++g_edge.simple_select0; }
     return;
   }
   depths_to_symbols(q1_cl_depth, 18, cl_bits);

@@ -96,6 +96,22 @@ class Oracle:
                                                C.byref(n), out) == 1
         return out.raw[:n.value]
 
+    def edge_stats_reset(self):
+        self.lib.oracle_edge_stats_reset()
+
+    def edge_stats(self):
+        """The entropy-stage edge counters since the last reset (oracle/brotli_oracle.c EDGE_FIELDS) as a dict."""
+        L = self.lib
+        L.oracle_edge_stats.restype = C.c_size_t
+        L.oracle_edge_stats.argtypes = [C.c_void_p, C.c_size_t]
+        L.oracle_edge_stats_names.restype = C.c_char_p
+        n = L.oracle_edge_stats(None, 0)
+        vals = (C.c_uint64 * n)()
+        L.oracle_edge_stats(vals, n)
+        names = L.oracle_edge_stats_names().decode().rstrip(",").split(",")
+        assert len(names) == n
+        return dict(zip(names, vals))
+
     def compress(self, data, quality, lgwin):
         n = len(data)
         cap = n + (n >> 1) + 4096
