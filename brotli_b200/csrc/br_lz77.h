@@ -91,10 +91,6 @@ BR_DEV u32 br_hash_key_v(const BrParams& P, u64 v) {
   if (P.hash64) return (u32)((v * (0x1FE35A7BD3579BD3ull << 24)) >> (64 - 15));
   return ((u32)v * 0x1E35A7BDu) >> (32 - P.bucket_bits);
 }
-#ifndef BR_WALK_SPEC1
-#define BR_WALK_SPEC1 0   /* G == 1: request the candidates' first bytes before their stored bit is known
-                             (timed on 100 MB of text: no gain, off) */
-#endif
 struct BrWalk {
   const BrStream* s;
   const u8* d;
@@ -236,6 +232,50 @@ BR_DEV void br_search_static_dict(BrWalk& w, u32 cur, u32 max_length, u32 max_ba
   }
 }
 
+// Entries of the bucket ring at search position `cur` (rank j) of a heavy bucket (slice [lo, hi) of S, hi - lo >= heavy_min).
+// The reference's per-bucket counter is a uint16 (hash_longest_match64_inc.h:52): after 65536 insertions it wraps and the
+// ring looks empty again.  c = insertions so far (of this stream).  Returns the number of entries the ring holds
+// (1 << block_bits unless the counter has wrapped to below that).
+// (Not skipped while the stream is shorter than 65536 bytes, although c cannot wrap there: the sensitivity this path
+// records -- min_wrap = 0 while the ring is not full -- also re-walks chunks whose view reached through their own freshly
+// unstored positions into a range that flipped in the same launch, which the successor count of br_commit_bits, taken over
+// the previous snapshot, could miss before it learnt to count with the runs' own fresh bits (k_cover): DESIGN.md
+// section 3, "the marking gap".  Kept: it costs nothing and is the net under that rule.)
+BR_DEV u32 br_ring_heavy(BrWalk& w, u32 j, u32 lo) {
+  const BrStream& s = *w.s;
+  const int lane = br_lane();
+  const u32 block_size = 1u << s.P.block_bits;
+  u32 lo_s = lo;
+  if (w.base) {   // batch of streams: the bucket's slice starts with the positions of the streams in front
+    u32 a = lo, b = j;
+    while (a < b) { const u32 mid = (a + b) >> 1; if (br_ldg(s.S + mid) < w.base) a = mid + 1; else b = mid; }
+    lo_s = a;
+  }
+  u32 own_cnt = 0, jj = j, n_own = 0;
+  BR_W(2, 1);
+  br_own_sync(w);
+  while (jj > lo) {
+    BR_W(3, 1);
+    u32 idx = jj - 1 - (u32)lane;
+    bool has = (jj >= lo + 1 + (u32)lane);
+    u32 q = has ? br_ldg(s.S + idx) : 0;
+    bool mine = has && q >= w.p0;
+    u32 mm = br_ballot(mine);
+    own_cnt += (u32)br_popc(br_ballot(mine && br_own_get(w, q)));
+    n_own += (u32)br_popc(mm);
+    if (mm != (BR_WARP == 32 ? 0xffffffffu : 1u)) break;
+    jj -= BR_WARP;
+  }
+  u32 jb = j - n_own;
+  u32 prev_cnt = br_countS_upto(s, jb) - br_countS_upto(s, lo_s);
+  u32 c = (prev_cnt + own_cnt) & 0xFFFFu;
+  if (c < block_size) { w.min_wrap = 0; return c; }
+  u32 sd = c - block_size, su = 65535u - c;
+  u32 m = sd < su ? sd : su;
+  if (m < w.min_wrap) w.min_wrap = m;
+  return block_size;
+}
+
 // FindLongestMatch (hash_longest_match64_inc.h:157, hash_longest_match_inc.h:156), lane-parallel:
 // every candidate's full match length is computed by its own lane, then the reference's
 // sequential "better than the best so far" rule is replayed with ballots.  The reference's
@@ -250,6 +290,11 @@ BR_DEV void br_search_static_dict(BrWalk& w, u32 cur, u32 max_length, u32 max_ba
 // loaded back to back, then their stored bits and the first 8 bytes of every candidate (speculatively, before the
 // stored bit is known), and only then the rows are folded in order: three round trips per G rows.  This is what a
 // latency-bound walker (a sweep, br_walk_block) needs; the fold itself is unchanged.
+//
+// G == 1 (quality 5-6: 4 distance-cache probes, 16- or 32-entry rings): a separate pass for the four distance-cache
+// candidates leaves 28 of 32 lanes idle.  So at quality 5 the first pass runs over 32 candidate slots
+// [distance cache ++ the newest 28 entries of the ring] -- the reference's order (hash.h:80 first, then the ring newest
+// first) -- with one match-length computation and one fold; further ring rows (32 entries each) follow from j - 28.
 template <int G>
 BR_DEV void br_find_longest_match(BrWalk& w, u32 cur, u32 max_length, u32 max_backward,
                                   u32 dict_distance, BrSR& out) {
@@ -266,124 +311,182 @@ BR_DEV void br_find_longest_match(BrWalk& w, u32 cur, u32 max_length, u32 max_ba
 #ifdef BR_DEBUG_KNOBS
   ++w.dbg_searches;
 #endif
-  bool brk = false;
   // the bytes at the search position, shared by every candidate comparison below
   const u64 c0 = br_ld64u(d, cur), c1 = br_ld64u(d, cur + 8);
   // Load order = latency plan.  (1) the index entry of `cur` (bucket bounds, rank) and the first bytes of the
   // distance-cache candidates are requested together; (2) the first G rows of the bucket's slice of S go out as soon
-  // as the rank is there, and the distance-cache fold runs while they are in flight; (3) stored bits + candidate
-  // bytes; (4) fold.  Three dependent round trips per search instead of one per step.
+  // as the rank is there (G > 1: the distance-cache fold runs while they are in flight; quality 5: the first row shares
+  // the distance cache's pass, and its snapshot bits go out with it); (3) stored bits + candidate bytes; (4) fold.
+  // Three dependent round trips per search instead of one per step.
   const u32 key = br_hash_key_v(P, c0);
   const u32 lo = br_ldg(s.seg + key), hi = br_ldg(s.seg + key + 1);
   const u32 j = br_ldg(s.rank + cur);
-  // ---- distance cache probes: lane k owns candidate k (hash.h:80 PrepareDistanceCache layout)
-  constexpr int ND = (16 + BR_WARP - 1) / BR_WARP;
-  u32 dback[ND]; u64 da0[ND]; bool dvalid[ND];
-#pragma unroll
-  for (int i = 0; i < ND; ++i) {
-    const int k = i * BR_WARP + lane;
-    int back_i = 0;
-    if (k < 4) back_i = k == 0 ? w.dc[0] : k == 1 ? w.dc[1] : k == 2 ? w.dc[2] : w.dc[3];
-    else if (k < 16) {   // dc[4..15] = last -1, +1, -2, +2, -3, +3; second last likewise (hash.h:83-97)
-      int mag = (int)((0xE79u >> (2 * ((k - 4) >> 1))) & 3u);
-      back_i = (k < 10 ? w.dc[0] : w.dc[1]) + ((k & 1) ? mag : -mag);
-    }
-    dvalid[i] = (k < P.ndist) && back_i > 0 && (u32)back_i <= max_backward;
-    dback[i] = (u32)back_i;
-    da0[i] = dvalid[i] ? br_ld64u(d, cur - (u32)back_i) : 0;
-  }
-  // first G rows of the bucket ring (consumed by the loop further down), with their tags
+  const u32 block_size = 1u << P.block_bits;
+  u32 V = block_size;   // ring entries the reference holds (fewer only in a heavy bucket whose counter wrapped)
+  u32 collected = 0, jj = j;   // stored ring entries seen so far; the ring's slice of S still to read is [lo, jj)
+  bool done = false;           // the ring ends (window, stream start, ring-buffer stop)
   const u32 tag_cur = br_tag4((u32)c0);
-  u32 q[G]; bool has[G], tagok[G];
+  u32 q[G] = {}; bool has[G] = {}, tagok[G] = {};   // the ring rows in flight (G > 1: the first G are loaded up front)
+  // The shared pass only where the whole ring fits in it (quality 5: 16 entries).  The 32-entry ring of quality 6 would
+  // need a second, dependent row after it: timed on 100 MB of text, that made the walk 22 % slower than a distance-cache
+  // pass that runs while the first full row is in flight.
+  if (G == 1 && block_size <= 28u) {
+    // ---- one pass over the 32 candidate slots k = [distance cache (hash.h:80, qualities 5-6 probe 4) ++ the newest
+    // 28 ring entries].  On the GPU lane k owns slot k; in the one-lane build (tests/sim) the same code is a loop over k.
+    constexpr int NDC = 4, NC = 32 / BR_WARP;
+    // slot's candidate position; its first 8 bytes (distance cache); valid / has; the word of the S-ordered snapshot bits
+    // that holds the entry's bit (ring)
+    u32 ca[NC]; u64 ca0[NC]; bool cv[NC]; u32 csw[NC];
 #pragma unroll
-  for (int r = 0; r < G; ++r) {
-    const u32 jr = j > (u32)(r * BR_WARP) ? j - (u32)(r * BR_WARP) : 0u;
-    has[r] = jr >= lo + 1 + (u32)lane;
-    q[r] = has[r] ? br_ldg(s.S + (jr - 1 - (u32)lane)) : 0;
-    tagok[r] = has[r] && (G == 1 || (u32)br_ldg(s.tagS + (jr - 1 - (u32)lane)) == tag_cur);   // (tags: deep rings only, see k_tags)
-  }
+    for (int i = 0; i < NC; ++i) {
+      const int k = i * BR_WARP + lane;
+      csw[i] = 0;
+      if (k < NDC) {
+        const int back = k == 0 ? w.dc[0] : k == 1 ? w.dc[1] : k == 2 ? w.dc[2] : w.dc[3];
+        cv[i] = back > 0 && (u32)back <= max_backward;
+        ca[i] = cur - (u32)back;
+        ca0[i] = cv[i] ? br_ld64u(d, ca[i]) : 0;
+      } else {
+        // The row of S and its snapshot bits are requested as soon as the rank is there, not after the bucket bounds: the
+        // row's address depends on j only, and the slots in front of the bucket's slice (entries of other buckets) are
+        // dropped once lo arrives.  The snapshot word is needed only when the row lies in front of the walker's own range
+        // (decided below from the row's positions), but requesting it now takes a memory round trip off the search.
+        const u32 rk = (u32)(k - NDC);   // ring entry rk, newest first
+        const u32 idx = j - 1 - rk;
+        u32 qs = 0;
+        if (j > rk) { qs = br_ldg(s.S + idx); csw[i] = br_ldg(s.storedS + (idx >> 5)); }
+        cv[i] = j >= lo + 1 + rk;
+        ca[i] = cv[i] ? qs : 0;
+        ca0[i] = 0;
+      }
+    }
+    if (hi - lo >= P.heavy_min) V = br_ring_heavy(w, j, lo);
+    br_own_sync(w);
+    BR_W(8, 1); BR_W(1, 1);
+#ifdef BR_DEBUG_KNOBS
+    ++w.dbg_rows;
+#endif
+    bool brk = false;
 #pragma unroll
-  for (int i = 0; i < ND; ++i) {
-    if (i * BR_WARP >= P.ndist || brk) break;
-    const int k = i * BR_WARP + lane;
-    const bool valid = dvalid[i];
-    const u32 back = dback[i];
-    u32 len = 0; int eqmax = 0;
-    if (valid) {
-      len = br_match_len_d0(d, cur - back, cur, max_length, c0, c1, da0[i]);
-      if (len == max_length) eqmax = (w.stale == (u32)br_ldg(d + (cur - back) + max_length));
+    for (int i = 0; i < NC; ++i) {
+      const int k = i * BR_WARP + lane;
+      const bool isdc = k < NDC;
+      const u32 a = ca[i];
+      // ring slots: stored bits as in the rows below (the newest ring entry is slot NDC's); rank among the stored ring
+      // entries, then the ring ends at the first entry outside the window or the slice
+      const bool inwin = !isdc && cv[i] && cur - a <= max_backward;
+      bool st;
+      if (br_shfl(a, NDC % BR_WARP) < w.p0) {
+        const u32 idx = j - 1 - (u32)(k - NDC);
+        st = inwin && ((csw[i] >> (idx & 31)) & 1u);
+      } else st = inwin && br_is_stored(w, a);
+      const u32 m = br_ballot(st);
+      const bool take = st && (collected + (u32)br_popc(m & br_lanemask_lt()) < V);
+      if (br_ballot(!isdc && !inwin) != 0) done = true;
+      collected += (u32)br_popc(m);
+      // one match length for every probed slot
+      u32 len = 0; int eqmax = 0;
+      if (isdc ? cv[i] : take) {
+        BR_W(9, isdc ? 0 : 1);
+        len = br_match_len_d0(d, a, cur, max_length, c0, c1, isdc ? ca0[i] : br_ld64u(d, a));
+        if (!isdc && len < 4) len = 0;
+        if (len == max_length) eqmax = (w.stale == (u32)br_ldg(d + a + max_length));
+      }
+      const u32 dist = cur - a;
+      u32 score;
+      if (isdc) {
+        score = 135u * len + BR_SCORE_BASE + 15u;
+        if (k != 0) score -= 39u + ((0x1CA10u >> (k & 0xE)) & 0xEu);
+      } else score = len ? BR_SCORE_BASE + 135u * len - 30u * br_log2floor(dist) : 0;
+      const bool lenok = isdc ? cv[i] && (len >= 3 || (len == 2 && k < 2)) : take && len != 0;
+      const u32 pm = (a - w.base) & rmask;
+      int last = -1;
+      while (!brk) {
+        // a distance-cache candidate still to come ends the whole search once cur_m + best_len passes the ring buffer
+        if (br_ballot(isdc && cv[i] && lane > last) != 0 && cur_m + best_len > rmask) { brk = done = true; break; }
+        // the ring compares against a best length of at least 3, and the same test with it ends the ring only
+        const u32 bl3 = best_len < 3 ? 3u : best_len, bl = isdc ? best_len : bl3;
+        const bool rstop = cur_m + bl3 > rmask;
+        if (rstop) done = true;
+        const bool ok = lenok && lane > last && !(!isdc && rstop) && !(pm + bl > rmask) &&
+                        (len > bl || (len == bl && bl == max_length && eqmax)) && score > best_score;
+        const u32 mm = br_ballot(ok);
+        if (!mm) break;
+        const int f = br_ffs(mm) - 1;
+        best_len = br_shfl(len, f); best_score = br_shfl(score, f);
+        out.len = best_len; out.distance = br_shfl(dist, f); out.score = best_score;
+        last = f;
+      }
     }
-    u32 score = 135u * len + BR_SCORE_BASE + 15u;
-    if (k != 0) score -= 39u + ((0x1CA10u >> (k & 0xE)) & 0xEu);
-    const bool lenok = valid && (len >= 3 || (len == 2 && k < 2));
-    const u32 pm = (cur - back - w.base) & rmask;
-    int last = -1;
-    for (;;) {
-      // candidates are examined in order; everything up to `last` has been decided
-      u32 pending = br_ballot(valid && lane > last);
-      if (!pending) break;
-      if (cur_m + best_len > rmask) { brk = true; break; }
-      bool ok = lenok && lane > last && !(pm + best_len > rmask) &&
-                (len > best_len || (len == best_len && best_len == max_length && eqmax)) && score > best_score;
-      u32 mm = br_ballot(ok);
-      if (!mm) break;
-      int f = br_ffs(mm) - 1;
-      best_len = br_shfl(len, f); best_score = br_shfl(score, f);
-      out.len = best_len; out.distance = br_shfl(back, f); out.score = best_score;
-      last = f;
+    jj = j > 32u - NDC ? j - (32u - NDC) : 0u;
+  } else {
+    // ---- distance cache probes: lane k owns candidate k (hash.h:80 PrepareDistanceCache layout)
+    constexpr int ND = (16 + BR_WARP - 1) / BR_WARP;
+    u32 dback[ND]; u64 da0[ND]; bool dvalid[ND];
+#pragma unroll
+    for (int i = 0; i < ND; ++i) {
+      const int k = i * BR_WARP + lane;
+      int back_i = 0;
+      if (k < 4) back_i = k == 0 ? w.dc[0] : k == 1 ? w.dc[1] : k == 2 ? w.dc[2] : w.dc[3];
+      else if (k < 16) {   // dc[4..15] = last -1, +1, -2, +2, -3, +3; second last likewise (hash.h:83-97)
+        int mag = (int)((0xE79u >> (2 * ((k - 4) >> 1))) & 3u);
+        back_i = (k < 10 ? w.dc[0] : w.dc[1]) + ((k & 1) ? mag : -mag);
+      }
+      dvalid[i] = (k < P.ndist) && back_i > 0 && (u32)back_i <= max_backward;
+      dback[i] = (u32)back_i;
+      da0[i] = dvalid[i] ? br_ld64u(d, cur - (u32)back_i) : 0;
     }
+    // first G rows of the bucket ring (consumed by the loop further down), with their tags (deep rings only, see k_tags)
+#pragma unroll
+    for (int r = 0; r < G; ++r) {
+      const u32 jr = j > (u32)(r * BR_WARP) ? j - (u32)(r * BR_WARP) : 0u;
+      has[r] = jr >= lo + 1 + (u32)lane;
+      q[r] = has[r] ? br_ldg(s.S + (jr - 1 - (u32)lane)) : 0;
+      tagok[r] = has[r] && (G == 1 || (u32)br_ldg(s.tagS + (jr - 1 - (u32)lane)) == tag_cur);
+    }
+    bool brk = false;
+#pragma unroll
+    for (int i = 0; i < ND; ++i) {
+      if (i * BR_WARP >= P.ndist || brk) break;
+      const int k = i * BR_WARP + lane;
+      const bool valid = dvalid[i];
+      const u32 back = dback[i];
+      u32 len = 0; int eqmax = 0;
+      if (valid) {
+        len = br_match_len_d0(d, cur - back, cur, max_length, c0, c1, da0[i]);
+        if (len == max_length) eqmax = (w.stale == (u32)br_ldg(d + (cur - back) + max_length));
+      }
+      u32 score = 135u * len + BR_SCORE_BASE + 15u;
+      if (k != 0) score -= 39u + ((0x1CA10u >> (k & 0xE)) & 0xEu);
+      const bool lenok = valid && (len >= 3 || (len == 2 && k < 2));
+      const u32 pm = (cur - back - w.base) & rmask;
+      int last = -1;
+      for (;;) {
+        // candidates are examined in order; everything up to `last` has been decided
+        u32 pending = br_ballot(valid && lane > last);
+        if (!pending) break;
+        if (cur_m + best_len > rmask) { brk = true; break; }
+        bool ok = lenok && lane > last && !(pm + best_len > rmask) &&
+                  (len > best_len || (len == best_len && best_len == max_length && eqmax)) && score > best_score;
+        u32 mm = br_ballot(ok);
+        if (!mm) break;
+        int f = br_ffs(mm) - 1;
+        best_len = br_shfl(len, f); best_score = br_shfl(score, f);
+        out.len = best_len; out.distance = br_shfl(back, f); out.score = best_score;
+        last = f;
+      }
+    }
+    if (hi - lo >= P.heavy_min) V = br_ring_heavy(w, j, lo);
   }
   if (best_len < 3) best_len = 3;
-  // ---- bucket ring
+  // ---- bucket ring (for G == 1: the rows after the first pass)
   {
-    const u32 block_size = 1u << P.block_bits;
-    u32 V = block_size;
-    if (hi - lo >= P.heavy_min) {
-      // The reference's per-bucket counter is a uint16 (hash_longest_match64_inc.h:52): after
-      // 65536 insertions it wraps and the ring looks empty again.  c = insertions so far (of this stream).
-      // (Not skipped while the stream is shorter than 65536 bytes, although c cannot wrap there: the sensitivity this
-      // path records -- min_wrap = 0 while the ring is not full -- also re-walks chunks whose view reached through their
-      // own freshly unstored positions into a range that flipped in the same launch, which the successor count of
-      // br_commit_bits, taken over the previous snapshot, could miss before it learnt to count with the runs' own fresh
-      // bits (k_cover): DESIGN.md section 3, "the marking gap".  Kept: it costs nothing and is the net under that rule.)
-      u32 lo_s = lo;
-      if (w.base) {   // batch of streams: the bucket's slice starts with the positions of the streams in front
-        u32 a = lo, b = j;
-        while (a < b) { const u32 mid = (a + b) >> 1; if (br_ldg(s.S + mid) < w.base) a = mid + 1; else b = mid; }
-        lo_s = a;
-      }
-      u32 own_cnt = 0, jj = j, n_own = 0;
-      BR_W(2, 1);
-      br_own_sync(w);
-      while (jj > lo) {
-        BR_W(3, 1);
-        u32 idx = jj - 1 - (u32)lane;
-        bool has = (jj >= lo + 1 + (u32)lane);
-        u32 q = has ? br_ldg(s.S + idx) : 0;
-        bool mine = has && q >= w.p0;
-        u32 mm = br_ballot(mine);
-        own_cnt += (u32)br_popc(br_ballot(mine && br_own_get(w, q)));
-        n_own += (u32)br_popc(mm);
-        if (mm != (BR_WARP == 32 ? 0xffffffffu : 1u)) break;
-        jj -= BR_WARP;
-      }
-      u32 jb = j - n_own;
-      u32 prev_cnt = br_countS_upto(s, jb) - br_countS_upto(s, lo_s);
-      u32 c = (prev_cnt + own_cnt) & 0xFFFFu;
-      if (c < block_size) { V = c; w.min_wrap = 0; }
-      else {
-        u32 sd = c - block_size, su = 65535u - c;
-        u32 m = sd < su ? sd : su;
-        if (m < w.min_wrap) w.min_wrap = m;
-      }
-    }
-    u32 collected = 0, jj = j;
-    bool done = false;
     br_own_sync(w);
     while (!done && collected < V && jj > lo) {
       u64 d0[G]; bool inwin[G], st[G];
       BR_W(8, 1);
-      // ---- fetch: G rows of S (the first G are already here), then their stored bits and (G > 1) the candidates' first bytes
+      // ---- fetch: G rows of S (the first G are already here unless the shared pass took the first row), then their
+      // stored bits and (G > 1) the candidates' first bytes
       if (jj != j) {
 #pragma unroll
         for (int r = 0; r < G; ++r) {
@@ -406,7 +509,7 @@ BR_DEV void br_find_longest_match(BrWalk& w, u32 cur, u32 max_length, u32 max_ba
           st[r] = inwin[r] && ((br_ldg(s.storedS + (idx >> 5)) >> (idx & 31)) & 1u);
         } else st[r] = inwin[r] && br_is_stored(w, q[r]);
       }
-      if (G > 1 || BR_WALK_SPEC1) {
+      if (G > 1) {
 #pragma unroll
         for (int r = 0; r < G; ++r) d0[r] = (inwin[r] && tagok[r]) ? br_ld64u(d, q[r]) : 0;
       }
@@ -432,7 +535,7 @@ BR_DEV void br_find_longest_match(BrWalk& w, u32 cur, u32 max_length, u32 max_ba
         u32 len = 0; int eqmax = 0;
         if (take && tagok[r]) {
           BR_W(9, 1);
-          len = (G > 1 || BR_WALK_SPEC1) ? br_match_len_d0(d, q[r], cur, max_length, c0, c1, d0[r]) : br_match_len_c(d, q[r], cur, max_length, c0, c1);
+          len = G > 1 ? br_match_len_d0(d, q[r], cur, max_length, c0, c1, d0[r]) : br_match_len_c(d, q[r], cur, max_length, c0, c1);
           if (len < 4) len = 0;
           if (len == max_length) eqmax = (w.stale == (u32)br_ldg(d + q[r] + max_length));
         }
