@@ -176,6 +176,21 @@ BR_DEV void br_commit_bits(const BrStream& s, u32 k) {
   }
 }
 
+// Qualities 5..9: carries the commits of a launch into the S-ordered snapshot the walkers read.  Between launches storedS
+// is bits_latest permuted into S order and cntS[b] counts its set bits in [1024 b, 1024 b + 1024) (prefS is the exclusive
+// scan of cntS).  bits_latest changes only in br_commit_bits, against the copy bits_prev taken before the commits, so the
+// bits q of word x that differ from bits_prev are exactly the entries rank[q] of storedS to flip.
+BR_DEV void br_snapshot_update(const BrStream& s, u32 x, u32* storedS, u32* cntS) {
+  u32 f = s.bits_latest[x] ^ s.bits_prev[x];
+  while (f) {
+    const u32 j = s.rank[(x << 5) + (u32)br_ffs(f) - 1u];
+    f &= f - 1;
+    const u32 b = 1u << (j & 31);
+    const u32 old = br_atomic_xor(storedS + (j >> 5), b);
+    br_atomic_add(cntS + (j >> 10), (old & b) ? 0xFFFFFFFFu : 1u);
+  }
+}
+
 // Qualities 2..4 (BrParams::quick): is the latest run of chunk k consistent with the committed stored-bits?  A slot of the
 // reference's table holds one position, so the run recorded what every search read from each slot (BrStream::saw,
 // br_find_quick): the index in S of the stored position it took, or BR_SAW_ABSENT | the index its backward walk

@@ -1,7 +1,7 @@
 // br_kernels.cu -- CUDA kernels (sm_90a) and the per-stream pipeline that drives them.
 //
 // Stage map (reference function -> kernel):
-//   hash keys / bucket rings (hash_longest_match64_inc.h Store*)  -> k_hash_keys, k_radix_* (the last pass writes rank[]), k_seg
+//   hash keys / bucket rings (hash_longest_match64_inc.h Store*)  -> br_build_index: k_radix_*, k_rank_compose, k_seg
 //   CreateBackwardReferences + FindLongestMatch                   -> k_walk      (one warp per input block)
 //   EncodeData glue (encode.c:985)                                -> k_chain     (one warp per stream)
 //   BrotliBuildMetaBlockGreedy + BrotliStoreMetaBlock             -> k_encode_mb (one warp per metablock)
@@ -26,12 +26,17 @@
   return 0; } } while (0)
 
 // ---------------------------------------------------------------------------- hashing + sort
-__global__ void k_hash_keys(BrParams P, const u8* __restrict__ data, u16* __restrict__ keys) {
-  u32 p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= P.n) return;
-  u32 hashable = P.n >= P.htl ? P.n - P.htl + 1 : 0;
-  keys[p] = (u16)(p < hashable ? br_hash_key(P, data, p) : P.nbuckets);
-}
+// Where a radix pass reads its keys: a materialised array, or (qualities 5..9, first pass) the bucket key computed from
+// the input on the fly, with the overflow key P.nbuckets for the unhashable tail.  A batch job (P.multi) hashes over the
+// whole concatenation, like a single stream.
+template <class KT> struct BrKeyArray {
+  const KT* k;
+  __device__ __forceinline__ u32 operator()(u32 j) const { return k[j]; }
+};
+struct BrKeyHash {
+  BrParams P; const u8* data; u32 hashable;
+  __device__ __forceinline__ u32 operator()(u32 j) const { return j < hashable ? br_hash_key(P, data, j) : P.nbuckets; }
+};
 
 // qualities 2..4: the key is the table slot of the one-position-per-slot hashers (br_lz77.h br_quick_slot), up to 20 bits
 // (+ the overflow key of the unhashable tail): 32-bit keys, three radix passes
@@ -51,62 +56,122 @@ __global__ void k_slot_pred(BrStream s, u32* __restrict__ qpred) {
     br_quick_pred_fill(s, p, B.base, qpred + ((size_t)p << s.P.qk_sweep_bits));
 }
 
-#define RADIX_TILE 4096
-// digit histogram of one tile -> hist[d * ntiles + tile]   (KT: u16 bucket keys, u32 slot keys)
-template <int SHIFT, class KT = u16>
-__global__ void __launch_bounds__(256) k_radix_count(const KT* __restrict__ keys, u32 n, u32* __restrict__ hist, u32 ntiles) {
+// Stable LSD radix sort, 8-bit digits.  A tile of RADIX_TILE elements is one CTA of RADIX_THREADS threads; warp w owns
+// the tile's elements [w * RADIX_ROWS * 32, (w + 1) * RADIX_ROWS * 32), row by row, which keeps equal digits in input order.
+#define RADIX_TILE 8192
+#define RADIX_THREADS 256
+#define RADIX_WARPS (RADIX_THREADS / 32)
+#define RADIX_ROWS (RADIX_TILE / RADIX_THREADS)
+// digit histogram of one tile -> hist[d * ntiles + tile]
+template <int SHIFT, class Keys>
+__global__ void __launch_bounds__(RADIX_THREADS) k_radix_count(Keys keys, u32 n, u32* __restrict__ hist, u32 ntiles) {
   __shared__ u32 cnt[256];
   cnt[threadIdx.x] = 0;
   __syncthreads();
-  u32 base = blockIdx.x * RADIX_TILE;
-  for (u32 i = threadIdx.x; i < RADIX_TILE; i += 256) {
-    u32 j = base + i;
-    if (j < n) atomicAdd(&cnt[(keys[j] >> SHIFT) & 0xFF], 1u);
+  const u32 base = blockIdx.x * RADIX_TILE, lane = threadIdx.x & 31;
+  for (u32 i = threadIdx.x; i < RADIX_TILE; i += RADIX_THREADS) {
+    const u32 j = base + i;
+    const u32 d = j < n ? (keys(j) >> SHIFT) & 0xFFu : 0xFFFFFFFFu;
+    const u32 m = __match_any_sync(0xffffffffu, d);   // one shared atomic per distinct digit of the row
+    if (d != 0xFFFFFFFFu && (m & ((1u << lane) - 1)) == 0) atomicAdd(&cnt[d], (u32)__popc(m));
   }
   __syncthreads();
   hist[threadIdx.x * ntiles + blockIdx.x] = cnt[threadIdx.x];
 }
-// stable scatter: warp w of the CTA owns elements [w*512, w*512+512) of the tile, row by row
-// `inv` (nullable): the final pass also writes the inverse permutation inv[position] = index in the sorted order (BrStream::rank)
-template <int SHIFT, bool HAS_VALS, class KT = u16>
-__global__ void __launch_bounds__(256) k_radix_scatter(const KT* __restrict__ keys, const u32* __restrict__ vals, u32 n,
-    const u32* __restrict__ hist_scanned, u32 ntiles, KT* __restrict__ out_keys, u32* __restrict__ out_vals, u32* __restrict__ inv) {
-  __shared__ u32 wcnt[8][256];
+static size_t radix_smem_bytes(size_t key_bytes) { return (RADIX_WARPS + 1) * 256 * 4 + RADIX_TILE * (4 + key_bytes); }
+// Stable scatter of one tile.  The tile is first reordered in shared memory into digit order; then consecutive threads
+// write each digit's run to consecutive addresses from hist_scanned[d * ntiles + tile] on, so the stores coalesce.
+// Values: vals[j], or the position j itself in a first pass (HAS_VALS false).
+// `rk` (nullable) gets rk[j] = the element's index in this pass's output, written by input index j (coalesced).  A first
+// pass's rk is the inverse permutation of its scatter by position; a later pass's rk may alias `vals`, because each index
+// j is read and then written by the same thread.  k_rank_compose chains them into BrStream::rank.
+// (Two CTAs per SM: the tile's keys stay in registers between the count and the placement.)
+template <int SHIFT, bool HAS_VALS, class KT, class Keys>
+__global__ void __launch_bounds__(RADIX_THREADS, 2) k_radix_scatter(Keys keys, const u32* vals, u32 n,
+    const u32* __restrict__ hist_scanned, u32 ntiles, KT* __restrict__ out_keys, u32* __restrict__ out_vals, u32* rk) {
+  extern __shared__ u32 smem[];
+  u32 (*wcnt)[256] = (u32 (*)[256])smem;         // per warp and digit: count, then the warp's first tile-local index
+  u32* gbase = smem + RADIX_WARPS * 256;           // per digit: output index of tile-local index 0
+  u32* sv = gbase + 256;                           // the tile in digit order: values ...
+  KT* sk = (KT*)(sv + RADIX_TILE);                 // ... and keys
   const u32 warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (u32 i = threadIdx.x; i < 8 * 256; i += 256) (&wcnt[0][0])[i] = 0;
+  for (u32 i = threadIdx.x; i < RADIX_WARPS * 256; i += RADIX_THREADS) smem[i] = 0;
   __syncthreads();
-  const u32 wbase = blockIdx.x * RADIX_TILE + warp * 512;
-  for (u32 r = 0; r < 16; ++r) {
-    u32 j = wbase + r * 32 + lane;
-    u32 d = j < n ? ((keys[j] >> SHIFT) & 0xFFu) : 0xFFFFFFFFu;
-    u32 m = __match_any_sync(0xffffffffu, d);
+  const u32 tbase = blockIdx.x * RADIX_TILE, wbase = warp * (RADIX_ROWS * 32);
+  u32 k[RADIX_ROWS];
+#pragma unroll
+  for (u32 r = 0; r < RADIX_ROWS; ++r) {
+    const u32 j = tbase + wbase + r * 32 + lane;
+    k[r] = j < n ? keys(j) : 0;
+  }
+#pragma unroll
+  for (u32 r = 0; r < RADIX_ROWS; ++r) {
+    const u32 j = tbase + wbase + r * 32 + lane;
+    const u32 d = j < n ? (k[r] >> SHIFT) & 0xFFu : 0xFFFFFFFFu;
+    const u32 m = __match_any_sync(0xffffffffu, d);
     if (d != 0xFFFFFFFFu && (m & ((1u << lane) - 1)) == 0) wcnt[warp][d] += __popc(m);
     __syncwarp();
   }
   __syncthreads();
-  {
-    u32 d = threadIdx.x;
-    u32 running = hist_scanned[d * ntiles + blockIdx.x];
-    for (u32 w = 0; w < 8; ++w) { u32 t = wcnt[w][d]; wcnt[w][d] = running; running += t; }
+  {  // thread d: the digit's tile-local start (exclusive scan over the digits), its output base and the warps' starts
+    __shared__ u32 wsum[RADIX_WARPS];
+    const u32 d = threadIdx.x;
+    u32 c = 0;
+    for (u32 w = 0; w < RADIX_WARPS; ++w) c += wcnt[w][d];
+    u32 x = c;
+    for (int o = 1; o < 32; o <<= 1) { const u32 t = __shfl_up_sync(0xffffffffu, x, o); if (lane >= (u32)o) x += t; }
+    if (lane == 31) wsum[warp] = x;
+    __syncthreads();
+    u32 start = x - c;
+    for (u32 w = 0; w < warp; ++w) start += wsum[w];
+    gbase[d] = hist_scanned[d * ntiles + blockIdx.x] - start;
+    for (u32 w = 0; w < RADIX_WARPS; ++w) { const u32 t = wcnt[w][d]; wcnt[w][d] = start; start += t; }
   }
   __syncthreads();
-  for (u32 r = 0; r < 16; ++r) {
-    u32 j = wbase + r * 32 + lane;
-    u32 k = j < n ? keys[j] : 0;
-    u32 d = j < n ? ((k >> SHIFT) & 0xFFu) : 0xFFFFFFFFu;
-    u32 m = __match_any_sync(0xffffffffu, d);
-    u32 rank = __popc(m & ((1u << lane) - 1));
+#pragma unroll
+  for (u32 r = 0; r < RADIX_ROWS; ++r) {
+    const u32 j = tbase + wbase + r * 32 + lane;
+    const u32 d = j < n ? (k[r] >> SHIFT) & 0xFFu : 0xFFFFFFFFu;
+    const u32 m = __match_any_sync(0xffffffffu, d);
+    const u32 before = __popc(m & ((1u << lane) - 1));
     if (j < n) {
-      u32 dst = wcnt[warp][d] + rank;
-      out_keys[dst] = (KT)k;
-      const u32 v = HAS_VALS ? vals[j] : j;
-      out_vals[dst] = v;
-      if (inv) inv[v] = dst;
+      const u32 loc = wcnt[warp][d] + before;
+      sk[loc] = (KT)k[r];
+      sv[loc] = HAS_VALS ? vals[j] : j;
+      if (rk) rk[j] = gbase[d] + loc;   // (after this thread's read of vals[j]: the only access to index j)
     }
     __syncwarp();
-    if (d != 0xFFFFFFFFu && rank == 0) wcnt[warp][d] += __popc(m);
+    if (d != 0xFFFFFFFFu && before == 0) wcnt[warp][d] += __popc(m);
     __syncwarp();
   }
+  __syncthreads();
+  const u32 len = n - tbase < RADIX_TILE ? n - tbase : RADIX_TILE;
+  for (u32 i = threadIdx.x; i < len; i += RADIX_THREADS) {
+    const u32 kk = sk[i];
+    const u32 dst = gbase[(kk >> SHIFT) & 0xFFu] + i;
+    out_keys[dst] = (KT)kk;
+    out_vals[dst] = sv[i];
+  }
+}
+// rank[p] = r_last[r_mid[rank[p]]] (r_mid nullable), in place: on entry rank holds the first pass's rk
+__global__ void k_rank_compose(u32* __restrict__ rank, const u32* __restrict__ r_mid, const u32* __restrict__ r_last, u32 n) {
+  const u32 p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  u32 i = rank[p];
+  if (r_mid) i = r_mid[i];
+  rank[p] = r_last[i];
+}
+static void scan_exclusive(u32* a, u32 n, u32* tmp, cudaStream_t st);
+// one radix pass: histogram, its scan, scatter
+template <int SHIFT, bool HAS_VALS, class KT, class Keys>
+static void radix_pass(Keys keys, const u32* vals, u32 n, u32* hist, u32* scan_tmp, KT* out_keys, u32* out_vals, u32* rk,
+                       cudaStream_t st) {
+  const u32 ntiles = (n + RADIX_TILE - 1) / RADIX_TILE;
+  const int smem = (int)radix_smem_bytes(sizeof(KT));
+  cudaFuncSetAttribute(k_radix_scatter<SHIFT, HAS_VALS, KT, Keys>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  k_radix_count<SHIFT><<<ntiles, RADIX_THREADS, 0, st>>>(keys, n, hist, ntiles);
+  scan_exclusive(hist, 256 * ntiles, scan_tmp, st);
+  k_radix_scatter<SHIFT, HAS_VALS, KT><<<ntiles, RADIX_THREADS, smem, st>>>(keys, vals, n, hist, ntiles, out_keys, out_vals, rk);
 }
 // chunk table of one input block (what br_build_blocks would fill on the host): one CTA per block
 __global__ void k_build_chunks(const BrBlk* __restrict__ blk, BrBlockIn* __restrict__ bin, u32 ch) {
@@ -131,6 +196,37 @@ __global__ void k_seg(const KT* __restrict__ sorted_keys, u32 n, u32 nbuckets, u
   int k0 = j == 0 ? -1 : (int)sorted_keys[j - 1];
   int k1 = j == n ? (int)nbuckets + 1 : (int)sorted_keys[j];
   for (int k = k0 + 1; k <= k1; ++k) seg[k] = j;
+}
+
+// Buffers of the position index (n elements each unless noted).  Qualities 5..9 use K1, V1, K2; qualities 2..4 the four
+// 32-bit arrays qk_*.
+struct BrIndexBufs {
+  u16 *K1, *K2;                              // K2: the sorted bucket keys (BrStream::skeys)
+  u32 *V1, *S, *rank, *seg;                  // seg: nbuckets + 2 words
+  u32 *hist, *scan_tmp;                      // 256 * ntiles words and scan_tmp_words of that
+  u32 *qk_keys, *qk_K1, *qk_V1, *qk_V2;
+};
+// S, rank and seg of the input (and K2 at qualities 5..9), queued on st.  blk / nblk: the input blocks (the slot keys of
+// qualities 2..4 count positions from BrBlk::base).
+static void br_build_index(const BrParams& P, const u8* data, const BrBlk* blk, u32 nblk, const BrIndexBufs& b, cudaStream_t st) {
+  const u32 n = P.n;
+  if (P.quick) {
+    // sorted by (slot, position): three stable 8-bit passes over 32-bit keys (slots have up to 20 bits + the overflow key);
+    // rank = r3[r2[inv1]]: the two later passes' rk alias the values they have read
+    k_slot_keys<<<nblk, 256, 0, st>>>(P, data, blk, b.qk_keys);
+    radix_pass<0, false>(BrKeyArray<u32>{b.qk_keys}, nullptr, n, b.hist, b.scan_tmp, b.qk_K1, b.qk_V1, b.rank, st);
+    radix_pass<8, true>(BrKeyArray<u32>{b.qk_K1}, b.qk_V1, n, b.hist, b.scan_tmp, b.qk_keys, b.qk_V2, b.qk_V1, st);
+    radix_pass<16, true>(BrKeyArray<u32>{b.qk_keys}, b.qk_V2, n, b.hist, b.scan_tmp, b.qk_K1, b.S, b.qk_V2, st);
+    k_rank_compose<<<(n + 255) / 256, 256, 0, st>>>(b.rank, b.qk_V1, b.qk_V2, n);
+    k_seg<u32><<<(n + 1 + 255) / 256, 256, 0, st>>>(b.qk_K1, n, P.nbuckets, b.seg);
+  } else {
+    // two passes over the 16-bit bucket keys, hashed from the input in the first; rank = r1[inv1], r1 aliasing V1
+    const BrKeyHash hk{P, data, n >= P.htl ? n - P.htl + 1 : 0};
+    radix_pass<0, false>(hk, nullptr, n, b.hist, b.scan_tmp, b.K1, b.V1, b.rank, st);
+    radix_pass<8, true>(BrKeyArray<u16>{b.K1}, b.V1, n, b.hist, b.scan_tmp, b.K2, b.S, b.V1, st);
+    k_rank_compose<<<(n + 255) / 256, 256, 0, st>>>(b.rank, nullptr, b.V1, n);
+    k_seg<u16><<<(n + 1 + 255) / 256, 256, 0, st>>>(b.K2, n, P.nbuckets, b.seg);
+  }
 }
 
 // ---------------------------------------------------------------------------- exclusive scan
@@ -192,7 +288,7 @@ __global__ void k_init_bits(BrStream s) {
     if (v) atomicOr(s.bits_latest + wi, v);
   }
 }
-// bits_latest permuted into S order + per-1024 popcounts
+// bits_latest permuted into S order + per-1024 popcounts: the first snapshot of a job (br_snapshot_update keeps it)
 __global__ void __launch_bounds__(1024) k_build_storedS(BrStream s, u32* __restrict__ storedS, u32* __restrict__ blockcnt) {
   __shared__ u32 wsum[32];
   u32 j = blockIdx.x * 1024 + threadIdx.x;
@@ -206,6 +302,11 @@ __global__ void __launch_bounds__(1024) k_build_storedS(BrStream s, u32* __restr
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     if (threadIdx.x == 0) blockcnt[blockIdx.x] = v;
   }
+}
+
+__global__ void k_snapshot_update(BrStream s, u32* __restrict__ storedS, u32* __restrict__ cntS) {
+  const u32 x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x < s.bits_words) br_snapshot_update(s, x, storedS, cntS);
 }
 
 // ---------------------------------------------------------------------------- warp-task kernels
@@ -538,9 +639,9 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
   const u32 cmd_stride = ch / 2 + 2;
   size_t need = 0;
   auto add = [&](size_t bytes) { need += (bytes + 255) & ~(size_t)255; };
-  add((size_t)n + 64); add(2ull * n + 4); add(2ull * n + 4); add(4ull * n); add(2ull * n + 4); add(4ull * n); add(4ull * n); add(2ull * n + 4);
+  add((size_t)n + 64); add(2ull * n + 4); add(4ull * n); add(2ull * n + 4); add(4ull * n); add(4ull * n); add(2ull * n + 4);
   add(256ull * ntiles * 4); add(scan_tmp_words(256ull * ntiles) * 4);
-  add((P.nbuckets + 4) * 4ull); add(nwords * 4); add(2 * nwords * 4); add(nwords * 4); add(nwords * 4); add(nwords * 4); add(nwords * 4); add(nwords * 4); add((nwords + 64) * 4); add(((size_t)n / 1024 + 8) * 4);
+  add((P.nbuckets + 4) * 4ull); add(nwords * 4); add(2 * nwords * 4); add(nwords * 4); add(nwords * 4); add(nwords * 4); add(nwords * 4); add(nwords * 4); add((nwords + 64) * 4); add(((size_t)n / 1024 + 8) * 4); add(((size_t)n / 1024 + 8) * 4);
   add(scan_tmp_words((size_t)n / 1024 + 8) * 4);
   add(nb * sizeof(BrBlockIn) * 2); add(nb * sizeof(BrBlockOut)); add((size_t)nb * cmd_stride * sizeof(BrCmd));
   for (int i = 0; i < 14; ++i) add(nb * 4ull + 64);
@@ -556,14 +657,14 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
   if (!job->arena.reserve(need)) return 0;
   BrArena& A = job->arena;
   u8* data = A.take<u8>((size_t)n + 64);
-  u16* keys = A.take<u16>((size_t)n + 2); u16* K1 = A.take<u16>((size_t)n + 2); u32* V1 = A.take<u32>(n);
+  u16* K1 = A.take<u16>((size_t)n + 2); u32* V1 = A.take<u32>(n);
   u16* K2 = A.take<u16>((size_t)n + 2); u32* S = A.take<u32>(n); u32* rank = A.take<u32>(n); u16* tagS = A.take<u16>((size_t)n + 2);
   u32* hist = A.take<u32>(256ull * ntiles); u32* scan_tmp = A.take<u32>(scan_tmp_words(256ull * ntiles));
   u32* seg = A.take<u32>(P.nbuckets + 4);
   u32* bits_latest = A.take<u32>(nwords); u32* bits_cur = A.take<u32>(2 * (size_t)nwords);
   u32* srch_latest = A.take<u32>(nwords); u32* srch_cur = A.take<u32>(nwords); u32* bits_prev = A.take<u32>(nwords);
   u32* cover_cur = A.take<u32>(nwords);
-  u32* storedS = A.take<u32>(nwords + 64); u32* prefS = A.take<u32>((size_t)n / 1024 + 8);
+  u32* storedS = A.take<u32>(nwords + 64); u32* prefS = A.take<u32>((size_t)n / 1024 + 8); u32* cntS = A.take<u32>((size_t)n / 1024 + 8);
   u32* scan_tmp2 = A.take<u32>(scan_tmp_words((size_t)n / 1024 + 8));
   BrBlockIn* bin = A.take<BrBlockIn>(nb); BrBlockIn* bin_used = A.take<BrBlockIn>(nb);
   BrBlockOut* bout = A.take<BrBlockOut>(nb);
@@ -632,30 +733,8 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
   CK(cudaMemsetAsync(bits_cur, 0, 2 * (size_t)nwords * 4, st));
 
   // ---- position index: S, rank, seg
-  if (P.quick) {
-    // sorted by (slot, position): three stable 8-bit passes over 32-bit keys (slots have up to 20 bits + the overflow key)
-    k_slot_keys<<<nblk, 256, 0, st>>>(P, data, d_blk, qk_keys);
-    k_radix_count<0, u32><<<ntiles, 256, 0, st>>>(qk_keys, n, hist, ntiles);
-    scan_exclusive(hist, 256 * ntiles, scan_tmp, st);
-    k_radix_scatter<0, false, u32><<<ntiles, 256, 0, st>>>(qk_keys, nullptr, n, hist, ntiles, qk_K1, qk_V1, nullptr);
-    k_radix_count<8, u32><<<ntiles, 256, 0, st>>>(qk_K1, n, hist, ntiles);
-    scan_exclusive(hist, 256 * ntiles, scan_tmp, st);
-    k_radix_scatter<8, true, u32><<<ntiles, 256, 0, st>>>(qk_K1, qk_V1, n, hist, ntiles, qk_keys, qk_V2, nullptr);
-    k_radix_count<16, u32><<<ntiles, 256, 0, st>>>(qk_keys, n, hist, ntiles);
-    scan_exclusive(hist, 256 * ntiles, scan_tmp, st);
-    k_radix_scatter<16, true, u32><<<ntiles, 256, 0, st>>>(qk_keys, qk_V2, n, hist, ntiles, qk_K1, S, rank);
-    k_seg<u32><<<(n + 1 + 255) / 256, 256, 0, st>>>(qk_K1, n, P.nbuckets, seg);
-    k_slot_pred<<<nblk, 256, 0, st>>>(s, qpred);   // (s.S / s.rank / s.seg / s.blk / s.data are set; the kernel reads nothing else)
-  } else {
-  k_hash_keys<<<(n + 255) / 256, 256, 0, st>>>(P, data, keys);
-  k_radix_count<0><<<ntiles, 256, 0, st>>>(keys, n, hist, ntiles);
-  scan_exclusive(hist, 256 * ntiles, scan_tmp, st);
-  k_radix_scatter<0, false><<<ntiles, 256, 0, st>>>(keys, nullptr, n, hist, ntiles, K1, V1, nullptr);
-  k_radix_count<8><<<ntiles, 256, 0, st>>>(K1, n, hist, ntiles);
-  scan_exclusive(hist, 256 * ntiles, scan_tmp, st);
-  k_radix_scatter<8, true><<<ntiles, 256, 0, st>>>(K1, V1, n, hist, ntiles, K2, S, rank);
-  k_seg<u16><<<(n + 1 + 255) / 256, 256, 0, st>>>(K2, n, P.nbuckets, seg);
-  }
+  br_build_index(P, data, d_blk, nblk, BrIndexBufs{K1, K2, V1, S, rank, seg, hist, scan_tmp, qk_keys, qk_K1, qk_V1, qk_V2}, st);
+  if (P.quick) k_slot_pred<<<nblk, 256, 0, st>>>(s, qpred);   // (s.S / s.rank / s.seg / s.blk / s.data are set; the kernel reads nothing else)
   // (the 16/32-entry rings of quality 5-6 gained nothing from tags when timed on C2, so only the deep rings of quality 7-9,
   // where most of the 256 ring entries are hash collisions whose bytes need not be fetched, use them)
   if (P.block_bits >= 6) k_tags<<<(n + 255) / 256, 256, 0, st>>>(data, S, n, tagS);
@@ -663,6 +742,17 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
   CK(cudaMemsetAsync(bits_latest, 0, nwords * 4, st));
   k_init_bits<<<nblk, 256, 0, st>>>(s);
   cudaEventRecord(ev[1], st);
+  // the S-ordered snapshot of the stored bits, for the bucket rings of quality 5..9: built once here, then carried along by
+  // k_snapshot_update after every launch's commits
+  const u32 nsnap = (n + 1023) / 1024;
+  auto refresh_prefS = [&]() {
+    cudaMemcpyAsync(prefS, cntS, nsnap * 4ull, cudaMemcpyDeviceToDevice, st);
+    scan_exclusive(prefS, nsnap, scan_tmp2, st);
+  };
+  if (!P.quick) {
+    k_build_storedS<<<nsnap, 1024, 0, st>>>(s, storedS, cntS);
+    refresh_prefS();
+  }
 
   // ---- LZ77 fixpoint
   u32* hp = job->h_pinned;
@@ -699,10 +789,6 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
       CK(cudaMemsetAsync(srch_cur, 0, nwords * 4, st));
       CK(cudaMemsetAsync(counters + 4, 0, 4, st));
       CK(cudaMemsetAsync(counters + 16, 0, 4, st));
-      if (!P.quick) {   // (the S-ordered copy of the stored bits serves the bucket rings of quality 5..9)
-        k_build_storedS<<<(n + 1023) / 1024, 1024, 0, st>>>(s, storedS, prefS);
-        scan_exclusive(prefS, (n + 1023) / 1024, scan_tmp2, st);
-      }
       cudaEventRecord(ev[6], st);
       const u32 wg = (n_sched + 3) / 4;
       if (P.quick) {
@@ -723,6 +809,10 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
       }
       k_commit<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s);
       if (P.quick) k_verify<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s);
+      else {
+        k_snapshot_update<<<(u32)((nwords + 255) / 256), 256, 0, st>>>(s, storedS, cntS);
+        refresh_prefS();
+      }
     }
     cudaEventRecord(ev[2], st);
 #ifdef BR_DEBUG_KNOBS
@@ -844,55 +934,53 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
   return 1;
 }
 
-// Debug / test hook: copies the position index of the last job to the host.
-extern "C" __attribute__((visibility("default"))) int br_debug_sort(int quality, int lgwin, const u8* h_in, u32 n, u32* h_S, u32* h_seg) {
+// Debug / test hooks: the position index of a one-stream job, built by br_build_index and copied to the host.
+// h_rank, h_keys (nullable): rank (n words) and the sorted keys (n words; the bucket keys of skeys at qualities 5..9, the
+// slot keys at qualities 2..4, whose one input block starts at 0).
+extern "C" __attribute__((visibility("default"))) int br_debug_index(int quality, int lgwin, const u8* h_in, u32 n, u32* h_S,
+                                                                    u32* h_seg, u32* h_rank, u32* h_keys) {
   BrParams P;
-  if (!br_derive_params(quality, lgwin, n, n, &P)) return 0;
-  if (P.quick) {   // qualities 2..4: the slot-sorted index (32-bit keys, three passes), one stream = one block from 0
-    u8* data; u32 *k0, *k1, *v1, *v2, *S, *rank, *hist, *tmp, *seg; BrBlk* blk;
-    const u32 ntiles = (n + RADIX_TILE - 1) / RADIX_TILE;
-    BrBlk B; memset(&B, 0, sizeof(B)); B.start = 0; B.end = n; B.base = 0; B.send = n;
-    CK(cudaMalloc(&data, (size_t)n + 64)); CK(cudaMemset(data, 0, (size_t)n + 64));
-    CK(cudaMemcpy(data, h_in, n, cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&blk, sizeof(BrBlk))); CK(cudaMemcpy(blk, &B, sizeof(BrBlk), cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&k0, 4ull * n + 16)); CK(cudaMalloc(&k1, 4ull * n + 16)); CK(cudaMalloc(&v1, 4ull * n + 16)); CK(cudaMalloc(&v2, 4ull * n + 16));
-    CK(cudaMalloc(&S, 4ull * n + 16)); CK(cudaMalloc(&rank, 4ull * n + 16)); CK(cudaMalloc(&hist, 1024ull * ntiles));
-    CK(cudaMalloc(&tmp, scan_tmp_words(256ull * ntiles) * 4)); CK(cudaMalloc(&seg, (P.nbuckets + 4) * 4ull));
-    k_slot_keys<<<1, 256>>>(P, data, blk, k0);
-    k_radix_count<0, u32><<<ntiles, 256>>>(k0, n, hist, ntiles);
-    scan_exclusive(hist, 256 * ntiles, tmp, 0);
-    k_radix_scatter<0, false, u32><<<ntiles, 256>>>(k0, nullptr, n, hist, ntiles, k1, v1, nullptr);
-    k_radix_count<8, u32><<<ntiles, 256>>>(k1, n, hist, ntiles);
-    scan_exclusive(hist, 256 * ntiles, tmp, 0);
-    k_radix_scatter<8, true, u32><<<ntiles, 256>>>(k1, v1, n, hist, ntiles, k0, v2, nullptr);
-    k_radix_count<16, u32><<<ntiles, 256>>>(k0, n, hist, ntiles);
-    scan_exclusive(hist, 256 * ntiles, tmp, 0);
-    k_radix_scatter<16, true, u32><<<ntiles, 256>>>(k0, v2, n, hist, ntiles, k1, S, rank);
-    k_seg<u32><<<(n + 1 + 255) / 256, 256>>>(k1, n, P.nbuckets, seg);
-    CK(cudaDeviceSynchronize());
-    CK(cudaMemcpy(h_S, S, 4ull * n, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(h_seg, seg, (P.nbuckets + 2) * 4ull, cudaMemcpyDeviceToHost));
-    cudaFree(data); cudaFree(blk); cudaFree(k0); cudaFree(k1); cudaFree(v1); cudaFree(v2); cudaFree(S); cudaFree(rank); cudaFree(hist); cudaFree(tmp); cudaFree(seg);
-    return 1;
-  }
-  u8* data; u16 *keys, *K1, *K2; u32 *V1, *S, *hist, *tmp, *seg;
+  if (n == 0 || !br_derive_params(quality, lgwin, n, n, &P)) return 0;
   const u32 ntiles = (n + RADIX_TILE - 1) / RADIX_TILE;
-  CK(cudaMalloc(&data, (size_t)n + 64)); CK(cudaMemset(data, 0, (size_t)n + 64));
-  CK(cudaMemcpy(data, h_in, n, cudaMemcpyHostToDevice));
-  CK(cudaMalloc(&keys, 2ull * n + 4)); CK(cudaMalloc(&K1, 2ull * n + 4)); CK(cudaMalloc(&K2, 2ull * n + 4));
-  CK(cudaMalloc(&V1, 4ull * n)); CK(cudaMalloc(&S, 4ull * n)); CK(cudaMalloc(&hist, 1024ull * ntiles));
-  CK(cudaMalloc(&tmp, scan_tmp_words(256ull * ntiles) * 4)); CK(cudaMalloc(&seg, (P.nbuckets + 4) * 4));
-  k_hash_keys<<<(n + 255) / 256, 256>>>(P, data, keys);
-  k_radix_count<0><<<ntiles, 256>>>(keys, n, hist, ntiles);
-  scan_exclusive(hist, 256 * ntiles, tmp, 0);
-  k_radix_scatter<0, false><<<ntiles, 256>>>(keys, nullptr, n, hist, ntiles, K1, V1, nullptr);
-  k_radix_count<8><<<ntiles, 256>>>(K1, n, hist, ntiles);
-  scan_exclusive(hist, 256 * ntiles, tmp, 0);
-  k_radix_scatter<8, true><<<ntiles, 256>>>(K1, V1, n, hist, ntiles, K2, S, nullptr);
-  k_seg<u16><<<(n + 1 + 255) / 256, 256>>>(K2, n, P.nbuckets, seg);
-  CK(cudaDeviceSynchronize());
-  CK(cudaMemcpy(h_S, S, 4ull * n, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(h_seg, seg, (P.nbuckets + 2) * 4ull, cudaMemcpyDeviceToHost));
-  cudaFree(data); cudaFree(keys); cudaFree(K1); cudaFree(K2); cudaFree(V1); cudaFree(S); cudaFree(hist); cudaFree(tmp); cudaFree(seg);
-  return 1;
+  BrBlk B; memset(&B, 0, sizeof(B)); B.start = 0; B.end = n; B.base = 0; B.send = n;
+  size_t need = 0;
+  auto add = [&](size_t bytes) { need += (bytes + 255) & ~(size_t)255; };
+  add((size_t)n + 64); add(sizeof(BrBlk)); add(4ull * n + 16); add(4ull * n + 16); add(4ull * n + 16); add(4ull * n + 16);
+  add(4ull * n + 16); add(4ull * n + 16); add(4ull * n + 16); add(4ull * n + 16); add(4ull * n + 16); add((P.nbuckets + 4) * 4ull);
+  add(1024ull * ntiles); add(scan_tmp_words(256ull * ntiles) * 4);
+  BrArena A;
+  if (!A.reserve(need)) return 0;
+  u8* data = A.take<u8>((size_t)n + 64); BrBlk* blk = A.take<BrBlk>(1);
+  BrIndexBufs b;
+  b.K1 = A.take<u16>((size_t)n + 8); b.K2 = A.take<u16>((size_t)n + 8); b.V1 = A.take<u32>((size_t)n + 4);
+  b.S = A.take<u32>((size_t)n + 4); b.rank = A.take<u32>((size_t)n + 4);
+  b.qk_keys = A.take<u32>((size_t)n + 4); b.qk_K1 = A.take<u32>((size_t)n + 4); b.qk_V1 = A.take<u32>((size_t)n + 4);
+  b.qk_V2 = A.take<u32>((size_t)n + 4); b.seg = A.take<u32>(P.nbuckets + 4);
+  b.hist = A.take<u32>(256ull * ntiles); b.scan_tmp = A.take<u32>(scan_tmp_words(256ull * ntiles));
+  int ok = 0;
+  std::vector<u16> k16;
+  if (!b.scan_tmp) goto done;
+  if (cudaMemset(data, 0, (size_t)n + 64) != cudaSuccess || cudaMemcpy(data, h_in, n, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(blk, &B, sizeof(BrBlk), cudaMemcpyHostToDevice) != cudaSuccess) goto done;
+  br_build_index(P, data, blk, 1, b, 0);
+  if (cudaDeviceSynchronize() != cudaSuccess) goto done;
+  if (cudaMemcpy(h_S, b.S, 4ull * n, cudaMemcpyDeviceToHost) != cudaSuccess ||
+      cudaMemcpy(h_seg, b.seg, (P.nbuckets + 2) * 4ull, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  if (h_rank && cudaMemcpy(h_rank, b.rank, 4ull * n, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  if (h_keys) {
+    if (P.quick) { if (cudaMemcpy(h_keys, b.qk_K1, 4ull * n, cudaMemcpyDeviceToHost) != cudaSuccess) goto done; }
+    else {
+      k16.resize(n);
+      if (cudaMemcpy(k16.data(), b.K2, 2ull * n, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+      for (u32 j = 0; j < n; ++j) h_keys[j] = k16[j];
+    }
+  }
+  ok = 1;
+done:
+  cudaGetLastError();
+  A.release();
+  return ok;
+}
+extern "C" __attribute__((visibility("default"))) int br_debug_sort(int quality, int lgwin, const u8* h_in, u32 n, u32* h_S, u32* h_seg) {
+  return br_debug_index(quality, lgwin, h_in, n, h_S, h_seg, nullptr, nullptr);
 }

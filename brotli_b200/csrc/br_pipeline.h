@@ -32,4 +32,6 @@ void* br_job_stream(BrJob*);
 int br_job_compress_device(BrJob* job, int quality, int lgwin, uint32_t size_hint,
                            const uint8_t* d_in, uint32_t n, const uint8_t** d_out, size_t* out_size, const BrCuts* cuts);
 int br_debug_sort(int quality, int lgwin, const uint8_t* h_in, uint32_t n, uint32_t* h_S, uint32_t* h_seg);
+int br_debug_index(int quality, int lgwin, const uint8_t* h_in, uint32_t n, uint32_t* h_S, uint32_t* h_seg, uint32_t* h_rank,
+                   uint32_t* h_keys);
 }

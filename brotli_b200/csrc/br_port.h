@@ -38,6 +38,7 @@ BR_DEV u32 br_match_any(u32 v) { return __match_any_sync(0xffffffffu, v); }
 BR_DEV void br_prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
 BR_DEV u32 br_atomic_or(u32* p, u32 v) { return atomicOr(p, v); }
 BR_DEV u32 br_atomic_and(u32* p, u32 v) { return atomicAnd(p, v); }
+BR_DEV u32 br_atomic_xor(u32* p, u32 v) { return atomicXor(p, v); }
 BR_DEV u32 br_atomic_add(u32* p, u32 v) { return atomicAdd(p, v); }
 BR_DEV int br_atomic_max(int* p, int v) { return atomicMax(p, v); }
 BR_DEV u32 br_atomic_min(u32* p, u32 v) { return atomicMin(p, v); }
@@ -87,6 +88,7 @@ BR_DEV u32 br_match_any(u32) { return 1u; }
 BR_DEV void br_prefetch_l2(const void*) {}
 BR_DEV u32 br_atomic_or(u32* p, u32 v) { u32 o = *p; *p = o | v; return o; }
 BR_DEV u32 br_atomic_and(u32* p, u32 v) { u32 o = *p; *p = o & v; return o; }
+BR_DEV u32 br_atomic_xor(u32* p, u32 v) { u32 o = *p; *p = o ^ v; return o; }
 BR_DEV u32 br_atomic_add(u32* p, u32 v) { u32 o = *p; *p = o + v; return o; }
 BR_DEV int br_atomic_max(int* p, int v) { int o = *p; if (v > o) *p = v; return o; }
 BR_DEV u32 br_atomic_min(u32* p, u32 v) { u32 o = *p; if (v < o) *p = v; return o; }
