@@ -20,6 +20,7 @@
 #include "br_assemble.h"
 #include "br_entropy_flat.h"
 #include "br_pipeline.h"
+#include "br_probe.h"
 
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { \
   fprintf(stderr, "brotli_b200: CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); \
@@ -983,4 +984,108 @@ done:
 }
 extern "C" __attribute__((visibility("default"))) int br_debug_sort(int quality, int lgwin, const u8* h_in, u32 n, u32* h_S, u32* h_seg) {
   return br_debug_index(quality, lgwin, h_in, n, h_S, h_seg, nullptr, nullptr);
+}
+
+// Test hook (tests/test_search_probe.py): one match search per probe (br_probe.h), one warp each, from a state the caller
+// specifies.  The index (br_build_index), tagS (k_tags), the S-ordered snapshot (k_build_storedS and its prefix) and, at
+// qualities 2..4, the slot entry points (k_slot_pred) are built by the pipeline's own kernels.
+template <int G>
+__global__ void k_search_probe(BrStream s, u32* own, const u32* probes, u32 np, u32* res) {
+  const u32 t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (t < np) br_probe_search<G>(s, own, probes + (size_t)t * BR_PROBE_WORDS, res + (size_t)t * BR_PROBE_WORDS);
+}
+// bounds[0 .. nstreams): the end of every stream of a batch laid end to end (bounds[nstreams - 1] == n; nstreams == 1: one
+// stream).  snap / own: the two stored-bit bitmaps, (n + 31) / 32 words each.  heavy_min: 0 keeps the pipeline's value.
+// probes are distinct positions (a quality 2..4 search records its slot reads per position).  res: BR_PROBE_WORDS words per
+// probe for every variant of the search, variant after variant: the pipeline's row grouping G, and at qualities 7..9 also
+// G = 1 and G = 8 (the fold does not depend on G).  tagS, storedS, prefS (nullable): n u16, (n + 31) / 32 words and
+// (n + 1023) / 1024 words.  Returns the number of variants (0: failure).
+extern "C" __attribute__((visibility("default"))) int br_debug_search(
+    int quality, int lgwin, int lgblock, u32 size_hint, const u8* h_in, u32 n, const u32* h_bounds, u32 nstreams,
+    const u32* h_snap, const u32* h_own, u32 heavy_min, const u32* h_probes, u32 np, u32* h_res, u16* h_tagS,
+    u32* h_storedS, u32* h_prefS) {
+  BrParams P;
+  if (n == 0 || nstreams == 0 || h_bounds[nstreams - 1] != n || !br_derive_params(quality, lgwin, size_hint, n, &P, lgblock)) return 0;
+  if (heavy_min) P.heavy_min = heavy_min;
+  if (nstreams > 1) P.multi = nstreams;
+  std::vector<u32> kinds(nstreams, 3);
+  std::vector<BrBlk> hblk;
+  u32 nb = 0;
+  br_build_blocks(P, n, h_bounds, nstreams - 1, true, nullptr, hblk, &nb, kinds.data());
+  const u32 nblk = (u32)hblk.size();
+  std::vector<u32> h_slot(((size_t)n >> P.lgblock) + 2, 0);
+  { u32 b = 0; for (size_t i = 0; i < h_slot.size(); ++i) { const u64 p = (u64)i << P.lgblock; while (b + 1 < nblk && hblk[b].end <= p) ++b; h_slot[i] = b; } }
+  BrDeviceTables* T = get_tables();
+  if (!T) return 0;
+  const int G[3] = {P.quick ? 0 : P.block_bits >= 6 ? BR_WALK_G_DEEP : BR_WALK_G_SMALL, 1, 8};
+  const int nvar = !P.quick && P.block_bits >= 6 ? 3 : 1;
+  const u32 ntiles = (n + RADIX_TILE - 1) / RADIX_TILE, nwords = (n + 31) / 32 + 2, nsnap = (n + 1023) / 1024;
+  const size_t nsaw = P.quick ? ((size_t)n << P.qk_sweep_bits) + 16 : 16;
+  size_t need = 1 << 16;
+  auto add = [&](size_t bytes) { need += (bytes + 255) & ~(size_t)255; };
+  add((size_t)n + 64); add(nblk * sizeof(BrBlk)); add(h_slot.size() * 4);
+  for (int i = 0; i < 9; ++i) add(4ull * n + 16);
+  add((P.nbuckets + 4) * 4ull); add(1024ull * ntiles); add(scan_tmp_words(256ull * ntiles) * 4);
+  add(2ull * n + 16); add(nwords * 4ull * 3 + 256); add(((size_t)n / 1024 + 8) * 8); add(scan_tmp_words((size_t)n / 1024 + 8) * 4);
+  add(nsaw * 8); add((size_t)np * BR_PROBE_WORDS * 4 * (1 + nvar));
+  BrArena A;
+  if (!A.reserve(need)) return 0;
+  u8* data = A.take<u8>((size_t)n + 64); BrBlk* blk = A.take<BrBlk>(nblk); u32* slot_blk = A.take<u32>(h_slot.size());
+  BrIndexBufs b;
+  b.K1 = A.take<u16>((size_t)n + 8); b.K2 = A.take<u16>((size_t)n + 8); b.V1 = A.take<u32>((size_t)n + 4);
+  b.S = A.take<u32>((size_t)n + 4); b.rank = A.take<u32>((size_t)n + 4);
+  b.qk_keys = A.take<u32>((size_t)n + 4); b.qk_K1 = A.take<u32>((size_t)n + 4); b.qk_V1 = A.take<u32>((size_t)n + 4);
+  b.qk_V2 = A.take<u32>((size_t)n + 4); b.seg = A.take<u32>(P.nbuckets + 4);
+  b.hist = A.take<u32>(256ull * ntiles); b.scan_tmp = A.take<u32>(scan_tmp_words(256ull * ntiles));
+  u16* tagS = A.take<u16>((size_t)n + 8);
+  u32* snap = A.take<u32>(nwords); u32* own = A.take<u32>(nwords); u32* storedS = A.take<u32>(nwords + 64);
+  u32* prefS = A.take<u32>((size_t)n / 1024 + 8); u32* cntS = A.take<u32>((size_t)n / 1024 + 8);
+  u32* scan_tmp2 = A.take<u32>(scan_tmp_words((size_t)n / 1024 + 8));
+  u32* qpred = A.take<u32>(nsaw); u32* saw = A.take<u32>(nsaw);
+  u32* probes = A.take<u32>((size_t)np * BR_PROBE_WORDS); u32* res = A.take<u32>((size_t)np * BR_PROBE_WORDS * nvar);
+  BrStream s; memset(&s, 0, sizeof(s));
+  int ok = 0;
+  if (!res) goto done;
+  s.P = P; s.data = data; s.S = b.S; s.rank = b.rank; s.seg = b.seg; s.skeys = b.K2; s.tagS = tagS;
+  s.bits_latest = snap; s.bits_words = nwords; s.storedS = storedS; s.prefS = prefS;
+  s.blk = blk; s.nblk = nblk; s.slot_blk = slot_blk; s.qpred = qpred; s.saw = saw;
+  { const u8* p = T->blob + 8;
+    s.dict_size_bits = p; p += 32; s.dict_offsets = (const u32*)p; p += 128; s.dict = p; p += 122784;
+    s.dict_hash_words = (const u16*)p; p += 65536; s.dict_hash_lengths = p; p += 32768; s.ctx_lut = p; }
+  s.log2tab = T->log2tab; s.log2tab_n = T->log2tab_n;
+  if (cudaMemset(data, 0, (size_t)n + 64) != cudaSuccess || cudaMemcpy(data, h_in, n, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(blk, hblk.data(), nblk * sizeof(BrBlk), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(slot_blk, h_slot.data(), h_slot.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemset(snap, 0, nwords * 4ull) != cudaSuccess || cudaMemset(own, 0, nwords * 4ull) != cudaSuccess ||
+      cudaMemcpy(snap, h_snap, (n + 31) / 32 * 4ull, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(own, h_own, (n + 31) / 32 * 4ull, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemset(saw, 0xEE, nsaw * 4) != cudaSuccess ||
+      cudaMemcpy(probes, h_probes, (size_t)np * BR_PROBE_WORDS * 4, cudaMemcpyHostToDevice) != cudaSuccess) goto done;
+  br_build_index(P, data, blk, nblk, b, 0);
+  if (P.quick) k_slot_pred<<<nblk, 256, 0>>>(s, qpred);
+  k_tags<<<(n + 255) / 256, 256>>>(data, b.S, n, tagS);
+  k_build_storedS<<<nsnap, 1024>>>(s, storedS, cntS);
+  if (cudaMemcpy(prefS, cntS, nsnap * 4ull, cudaMemcpyDeviceToDevice) != cudaSuccess) goto done;
+  scan_exclusive(prefS, nsnap, scan_tmp2, 0);
+  for (int v = 0; v < nvar; ++v) {
+    u32* r = res + (size_t)v * np * BR_PROBE_WORDS;
+    const u32 grid = (np + 3) / 4;
+    switch (G[v]) {
+      case 0: k_search_probe<0><<<grid, 128>>>(s, own, probes, np, r); break;
+      case 1: k_search_probe<1><<<grid, 128>>>(s, own, probes, np, r); break;
+      case 4: k_search_probe<4><<<grid, 128>>>(s, own, probes, np, r); break;
+      case 8: k_search_probe<8><<<grid, 128>>>(s, own, probes, np, r); break;
+      default: goto done;
+    }
+  }
+  if (cudaDeviceSynchronize() != cudaSuccess ||
+      cudaMemcpy(h_res, res, (size_t)np * BR_PROBE_WORDS * 4 * nvar, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  if (h_tagS && cudaMemcpy(h_tagS, tagS, 2ull * n, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  if (h_storedS && cudaMemcpy(h_storedS, storedS, (n + 31) / 32 * 4ull, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  if (h_prefS && cudaMemcpy(h_prefS, prefS, nsnap * 4ull, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  ok = nvar;
+done:
+  cudaGetLastError();
+  A.release();
+  return ok;
 }

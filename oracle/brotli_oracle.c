@@ -65,12 +65,19 @@ double oracle_fast_log2(size_t v) { return fast_log2(v); }
  *   ctx_nc1/2/3/13: compressed metablocks (quality 4+) by literal context count; lit_cap_nc*: those whose literal
  *       split reached the 256 / nc type cap; split_back: blocks merged into the type before last (action 2)
  *   max_lit_types / max_lit_trees / max_cmd_types / max_dist_types: per metablock
- *   max_insert / max_copy / max_block_len / max_distance: the longest emitted (distance: explicit codes only) */
+ *   max_insert / max_copy / max_block_len / max_distance: the longest emitted (distance: explicit codes only)
+ * The same for the match search (find_longest_match, tests/test_search_probe.py):
+ *   srch_dc_len2: searches won by a len-2 distance-cache match; srch_ring_break: the ring-buffer stop
+ *       (cur_m + best_len > rmask); srch_ring_skip: a candidate skipped by prev_m + best_len > rmask;
+ *   srch_tie_max: a candidate as long as a best length that already equals max_length (the stale byte decides);
+ *   srch_wrap_cut: a ring cut short by a wrapped uint16 counter (oracle_search_probe);
+ *   srch_dict_hit: a static-dictionary item taken; srch_gate_closed: the dictionary gate (hash.h:186) closed */
 #define EDGE_FIELDS(X) X(retry_lit) X(retry_cmd) X(retry_dist) X(retry_other) X(retry_cl) X(retry_fast) \
   X(simple_nsym1) X(simple_nsym2) X(simple_nsym3) X(simple_nsym4) X(simple_select0) X(simple_select1) X(rle_lt16) X(rle_lt28) X(rle_full) X(rle_holes) \
   X(reps7) X(reps11) X(rle_use_nz) X(rle_use_z) X(ctx_nc1) X(ctx_nc2) X(ctx_nc3) X(ctx_nc13) X(lit_cap_nc1) \
   X(lit_cap_nc2) X(lit_cap_nc3) X(lit_cap_nc13) X(split_back) X(max_lit_types) X(max_lit_trees) X(max_cmd_types) \
-  X(max_dist_types) X(max_insert) X(max_copy) X(max_block_len) X(max_distance)
+  X(max_dist_types) X(max_insert) X(max_copy) X(max_block_len) X(max_distance) \
+  X(srch_dc_len2) X(srch_ring_break) X(srch_ring_skip) X(srch_tie_max) X(srch_wrap_cut) X(srch_dict_hit) X(srch_gate_closed)
 #define EDGE_MEMBER(f) uint64_t f;
 #define EDGE_NAME(f) #f ","
 static struct { EDGE_FIELDS(EDGE_MEMBER) } g_edge;
@@ -333,14 +340,16 @@ static int test_dict_item(size_t len, size_t word_idx, const uint8_t* data,
 static void search_static_dict_n(Enc* e, const uint8_t* data, size_t max_length,
     size_t max_backward, size_t max_distance, SR* out, size_t probes) {
   size_t key, i;
-  if (e->dict_matches < (e->dict_lookups >> 7)) return;
+  if (e->dict_matches < (e->dict_lookups >> 7)) { ++g_edge.srch_gate_closed; return; }
   key = ((load32(data) * 0x1E35A7BDu) >> (32 - 14)) << 1;
   for (i = 0; i < probes; ++i, ++key) {
     e->dict_lookups++;
     if (g_hash_lengths[key] != 0) {
       if (test_dict_item(g_hash_lengths[key], g_hash_words[key], data,
-                         max_length, max_backward, max_distance, out))
+                         max_length, max_backward, max_distance, out)) {
         e->dict_matches++;
+        ++g_edge.srch_dict_hit;
+      }
     }
   }
 }
@@ -439,9 +448,10 @@ static void find_longest_match(Enc* e, size_t cur, size_t max_length,
     if (prev >= cur) continue;
     if (backward > max_backward) continue;
     prev_m = prev & rmask;
-    if (cur_m + best_len > rmask) break;
-    if (prev_m + best_len > rmask ||
-        cur_byte(e, cur, best_len, max_length) != data[prev + best_len]) continue;
+    if (cur_m + best_len > rmask) { ++g_edge.srch_ring_break; break; }
+    if (prev_m + best_len > rmask) { ++g_edge.srch_ring_skip; continue; }
+    if (best_len == max_length && match_len(data + prev, data + cur, max_length) == max_length) ++g_edge.srch_tie_max;
+    if (cur_byte(e, cur, best_len, max_length) != data[prev + best_len]) continue;
     len = match_len(data + prev, data + cur, max_length);
     if (len >= 3 || (len == 2 && i < 2)) {
       size_t score = score_last(len);
@@ -454,6 +464,7 @@ static void find_longest_match(Enc* e, size_t cur, size_t max_length,
       }
     }
   }
+  if (out->len == 2) ++g_edge.srch_dc_len2;
   if (best_len < 3) best_len = 3;
   {
     size_t nk = e->num[key];
@@ -464,8 +475,9 @@ static void find_longest_match(Enc* e, size_t cur, size_t max_length,
       int eq = 1;
       if (backward > max_backward) break;
       prev_m = prev & rmask;
-      if (cur_m + best_len > rmask) break;
-      if (prev_m + best_len > rmask) continue;
+      if (cur_m + best_len > rmask) { ++g_edge.srch_ring_break; break; }
+      if (prev_m + best_len > rmask) { ++g_edge.srch_ring_skip; continue; }
+      if (best_len == max_length && match_len(data + prev, data + cur, max_length) == max_length) ++g_edge.srch_tie_max;
       /* 4 bytes ending at best_len (hash_longest_match64_inc.h:246,
          hash_longest_match_inc.h:243) */
       for (k = 0; k < 4; ++k)
@@ -1521,6 +1533,39 @@ static void extend_last_command(Enc* e, size_t* bytes, size_t* pos) {
   }
 }
 
+/* Block size, hasher and ring buffer of an encoder for (quality, lgwin, BROTLI_PARAM_LGBLOCK (0: the encoder's choice),
+   BROTLI_PARAM_SIZE_HINT); returns MaxMetablockSize. */
+static size_t setup_hasher(Enc* e, int quality, int lgwin, int lgblock_user, size_t size_hint) {
+  e->quality = quality; e->lgwin = lgwin; e->size_hint = size_hint;
+  /* quality.h:75 ComputeLgBlock */
+  e->lgblock = quality < 4 ? 14 : 16;
+  if (quality >= 9 && lgwin > 16) e->lgblock = lgwin < 18 ? lgwin : 18;
+  if (lgblock_user && quality >= 4) e->lgblock = lgblock_user > 24 ? 24 : lgblock_user < 16 ? 16 : lgblock_user;
+  if (quality < 5) {
+    /* quality.h:172 ChooseHasher: H2, H3, H4, and H54 for quality 4 on inputs >= 1 MiB (hash.h:251-338) */
+    e->quick = 1; e->qk_hash_len = 5;
+    if (quality == 2) { e->qk_bits = 16; e->qk_sweep_bits = 0; e->qk_dict = 1; }
+    else if (quality == 3) { e->qk_bits = 16; e->qk_sweep_bits = 1; e->qk_dict = 0; }
+    else if (size_hint >= (1u << 20)) { e->qk_bits = 20; e->qk_sweep_bits = 2; e->qk_dict = 0; e->qk_hash_len = 7; }
+    else { e->qk_bits = 17; e->qk_sweep_bits = 2; e->qk_dict = 1; }
+    e->qk_table = (uint32_t*)calloc((size_t)1 << e->qk_bits, 4);
+    e->ndist = 1;
+    e->hash_type_len = 8; e->store_lookahead = 8;
+  } else {
+    e->hash64 = (size_hint >= (1u << 20) && lgwin >= 19);
+    e->block_bits = quality - 1;
+    e->bucket_bits = e->hash64 ? 15 : (quality < 7 ? 14 : 15);
+    e->ndist = quality < 7 ? 4 : quality < 9 ? 10 : 16;
+    e->hash_type_len = e->hash64 ? 8 : 4;
+    e->store_lookahead = e->hash_type_len;
+    e->num = (uint16_t*)calloc((size_t)1 << e->bucket_bits, 2);
+    e->buckets = (uint32_t*)calloc((size_t)1 << (e->bucket_bits + e->block_bits), 4);
+  }
+  { int rb = 1 + (lgwin > e->lgblock ? lgwin : e->lgblock);
+    e->rmask = ((size_t)1 << rb) - 1;
+    return (size_t)1 << (rb < 24 ? rb : 24); }
+}
+
 /* One-shot driver: encode.c:1296 BrotliEncoderCompress ->
    :1634 CompressStream(FINISH) -> :985 EncodeData per input block. */
 static int oracle_compress_impl(int quality, int lgwin, size_t n, const uint8_t* in,
@@ -1531,34 +1576,9 @@ static int oracle_compress_impl(int quality, int lgwin, size_t n, const uint8_t*
   if (quality >= 5 ? lgwin < 17 : lgwin < 10) return 0;      /* lgwin <= 16 at quality 5+: H40..42, not restated */
   if (n == 0) { if (*out_n < 1) return 0; out[0] = 6; *out_n = 1; return 1; }
   memset(&e, 0, sizeof(e));
-  e.quality = quality; e.lgwin = lgwin; e.size_hint = n; e.data = in; e.n = n;
+  e.data = in; e.n = n;
   e.cmd_hook = hook;
-  /* quality.h:75 ComputeLgBlock */
-  e.lgblock = quality < 4 ? 14 : 16;
-  if (quality >= 9 && lgwin > 16) e.lgblock = lgwin < 18 ? lgwin : 18;
-  if (quality < 5) {
-    /* quality.h:172 ChooseHasher: H2, H3, H4, and H54 for quality 4 on inputs >= 1 MiB (hash.h:251-338) */
-    e.quick = 1; e.qk_hash_len = 5;
-    if (quality == 2) { e.qk_bits = 16; e.qk_sweep_bits = 0; e.qk_dict = 1; }
-    else if (quality == 3) { e.qk_bits = 16; e.qk_sweep_bits = 1; e.qk_dict = 0; }
-    else if (n >= (1u << 20)) { e.qk_bits = 20; e.qk_sweep_bits = 2; e.qk_dict = 0; e.qk_hash_len = 7; }
-    else { e.qk_bits = 17; e.qk_sweep_bits = 2; e.qk_dict = 1; }
-    e.qk_table = (uint32_t*)calloc((size_t)1 << e.qk_bits, 4);
-    e.ndist = 1;
-    e.hash_type_len = 8; e.store_lookahead = 8;
-  } else {
-    e.hash64 = (n >= (1u << 20) && lgwin >= 19);
-    e.block_bits = quality - 1;
-    e.bucket_bits = e.hash64 ? 15 : (quality < 7 ? 14 : 15);
-    e.ndist = quality < 7 ? 4 : quality < 9 ? 10 : 16;
-    e.hash_type_len = e.hash64 ? 8 : 4;
-    e.store_lookahead = e.hash_type_len;
-    e.num = (uint16_t*)calloc((size_t)1 << e.bucket_bits, 2);
-    e.buckets = (uint32_t*)calloc((size_t)1 << (e.bucket_bits + e.block_bits), 4);
-  }
-  { int rb = 1 + (lgwin > e.lgblock ? lgwin : e.lgblock);
-    e.rmask = ((size_t)1 << rb) - 1;
-    max_mb = (size_t)1 << (rb < 24 ? rb : 24); }
+  max_mb = setup_hasher(&e, quality, lgwin, 0, n);
   e.dist_cache[0] = 4; e.dist_cache[1] = 11; e.dist_cache[2] = 15; e.dist_cache[3] = 16;
   memcpy(e.saved_dist_cache, e.dist_cache, 16);
   e.cmds = (Cmd*)malloc(sizeof(Cmd) * (max_mb / 2 + (1u << e.lgblock) + 64));
@@ -1710,4 +1730,79 @@ int oracle_brotli_compress_hook(int quality, int lgwin, size_t n, const uint8_t*
     size_t* out_n, uint8_t* out, void (*hook)(const void*, size_t, size_t, size_t)) {
   return oracle_compress_impl(quality, lgwin, n, in, out_n, out,
       (void (*)(const Cmd*, size_t, size_t, size_t))hook);
+}
+
+/* tests/test_search_probe.py: one FindLongestMatch per probe, from a fully specified hash-table state.
+ * data: one stream (n bytes, followed by at least 16 readable bytes); snap / own: one byte per position of the stream, the
+ * stored bits of the two bitmaps.  Position q counts as inserted in front of a search when q >= p0 ? own[q] : snap[q].
+ * probes (16 words each, ascending cur): cur, p0, base, pend, max_backward, dict_distance, dc[0..3], len_in, score_in,
+ * dict_l (lo, hi), dict_m (lo, hi).  Positions count from the batch's first byte: the stream starts at `base`.
+ * res (16 words each): len, distance, score, delta, dict lookups and matches added, gate checks, gate closed, whether cur
+ * was inserted, whether it was searched; the rest zero.
+ * Before each search the probe's stream is hashed into a fresh table in position order: every inserted q < cur.  Only
+ * the bucket (H5 / H6) or the slots (quick hashers) the search reads can affect it, so only the positions filed there are
+ * inserted.  The insertion of cur that the search makes is undone afterwards. */
+int oracle_search_probe(int quality, int lgwin, int lgblock, size_t size_hint, const uint8_t* data, size_t n,
+                        const uint8_t* snap, const uint8_t* own, const uint32_t* probes, size_t nprobes, uint32_t* res) {
+  Enc e; size_t i, nkeys, hashable;
+  uint32_t *start, *pos;
+  if (!g_blob || quality < 2 || quality > 9) return 0;
+  memset(&e, 0, sizeof(e));
+  e.data = data; e.n = n;
+  setup_hasher(&e, quality, lgwin, lgblock, size_hint);
+  /* positions by bucket / slot (counting sort); the last HashTypeLength - 1 are never inserted */
+  nkeys = e.quick ? (size_t)1 << e.qk_bits : (size_t)1 << e.bucket_bits;
+  hashable = n >= e.hash_type_len ? n - e.hash_type_len + 1 : 0;
+  start = (uint32_t*)calloc(nkeys + 2, 4); pos = (uint32_t*)malloc(4 * (hashable + 1));
+  {
+    uint32_t* key = (uint32_t*)malloc(4 * (hashable + 1));
+    const size_t qmask = ((size_t)1 << e.qk_bits) - 1;
+    for (i = 0; i < hashable; ++i) {
+      key[i] = (uint32_t)(e.quick ? (quick_key(&e, i) + (i & (((1u << e.qk_sweep_bits) - 1u) << 3))) & qmask : hash_key(&e, i));
+      ++start[key[i] + 2];
+    }
+    for (i = 2; i < nkeys + 2; ++i) start[i] += start[i - 1];
+    for (i = 0; i < hashable; ++i) pos[start[key[i] + 1]++] = (uint32_t)i;
+    free(key);
+  }
+  for (i = 0; i < nprobes; ++i) {
+    const uint32_t* pr = probes + 16 * i;
+    uint32_t* r = res + 16 * i;
+    const size_t base = pr[2], cur = pr[0] - base, p0 = pr[1] > base ? pr[1] - base : 0, pend = pr[3] - base;
+    const size_t block_size = (size_t)1 << e.block_bits;
+    const uint64_t dict_l = ((uint64_t)pr[13] << 32) | pr[12], dict_m = ((uint64_t)pr[15] << 32) | pr[14];
+    const uint64_t closed0 = g_edge.srch_gate_closed;
+    size_t keys[4], nk = 0, k, j, key = 0;
+    SR sr;
+    if (e.quick) {
+      const size_t sweep = (size_t)1 << e.qk_sweep_bits, mask = ((size_t)1 << e.qk_bits) - 1;
+      key = quick_key(&e, cur);
+      for (k = 0; k < sweep; ++k) { keys[nk++] = (key + (k << 3)) & mask; e.qk_table[keys[k]] = 0; }
+    } else {
+      key = hash_key(&e, cur);
+      keys[nk++] = key; e.num[key] = 0;
+    }
+    for (k = 0; k < nk; ++k) {
+      size_t c = 0;
+      for (j = start[keys[k]]; j < start[keys[k] + 1] && pos[j] < cur; ++j) {
+        const size_t q = pos[j];
+        if (q >= p0 ? own[q] : snap[q]) { hstore(&e, q); ++c; }
+      }
+      if (!e.quick && c >= 65536 && (c & 0xFFFF) < block_size) ++g_edge.srch_wrap_cut;
+    }
+    for (k = 0; k < 4; ++k) e.dist_cache[k] = (int)pr[6 + k];
+    prepare_dist_cache(e.dist_cache, e.ndist);
+    e.dict_lookups = (size_t)dict_l; e.dict_matches = (size_t)dict_m;
+    sr.len = pr[10]; sr.score = pr[11]; sr.distance = 0; sr.len_code_delta = 0;
+    find_longest_match(&e, cur, pend - cur, pr[4], pr[5], 0x3FFFFFC, &sr);
+    if (!e.quick) --e.num[key];   /* (the quick hashers' slots are refilled by the next probe) */
+    memset(r, 0, 16 * 4);
+    r[0] = (uint32_t)sr.len; r[1] = (uint32_t)sr.distance; r[2] = (uint32_t)sr.score; r[3] = (uint32_t)sr.len_code_delta;
+    r[4] = (uint32_t)(e.dict_lookups - dict_l); r[5] = (uint32_t)(e.dict_matches - dict_m);
+    r[7] = (uint32_t)(g_edge.srch_gate_closed - closed0);
+    r[6] = r[7] + (r[4] != 0);
+    r[8] = r[9] = 1;
+  }
+  free(start); free(pos); free(e.num); free(e.buckets); free(e.qk_table);
+  return 1;
 }
