@@ -276,6 +276,35 @@ BR_DEV u32 br_ring_heavy(BrWalk& w, u32 j, u32 lo) {
   return block_size;
 }
 
+// Lookahead of the quality 5 search (the shared pass below): L2 prefetch hints for the searches still to come, issued
+// while the current search waits on its own loads.  A search waits on three dependent round trips -- (bytes at cur, rank)
+// -> (row of S, its snapshot bits) -> candidates' first bytes -- and the last two are random reads of 400 MB and of the
+// 4 MB window that miss L2.  Their addresses for the next searches do not depend on the current search's result, only on
+// their positions, which the walker predicts (br_walk_one).  So:
+//   stage 1, BR_WALK1_LOOKAHEAD searches ahead: prefetch the row of S and its snapshot words;
+//   stage 2 (lookahead >= 2), the next search: load its row (now from L2) and prefetch the first bytes of its newest
+//   block_size entries inside the window.
+// Nothing loaded here reaches a search: every search still does all its own loads, which then hit L2.  A wrong prediction
+// costs memory traffic only.  0 turns the lookahead off; the one-lane CPU build (tests/sim) has none.
+// The walk is as much issue bound as latency bound (DESIGN.md section 3), so every instruction added here has to pay for
+// itself.  Timed on 100 MB of text at quality 5 (H100, section 5): lookahead 1 walks about 5 % faster than none; 2 and 3
+// (stage 2, in either of two forms) were slower than 1, and a prefetch of the bucket bounds seg[key] (a table L2 already
+// holds) cost more than it saved.
+#ifndef BR_WALK1_LOOKAHEAD
+#define BR_WALK1_LOOKAHEAD 1
+#endif
+struct BrLook {
+  u32 next;     // stage 2: the next search's position (~0u: none)
+  u32 f0, nf;   // stage 1: the rows of positions f0 .. f0 + nf - 1 (nf <= BR_WALK1_LOOKAHEAD)
+};
+// Position of the search that follows a FAILED search at x (br_walk_one's rule: x + 1, or the random-heuristics jump
+// past the literals; its clamp at the block end is left out, a prediction only has to be right most of the time).
+BR_DEV u32 br_next_search(u32 x, u32 apply_rh, u32 window) {
+  const u32 p = x + 1;
+  if (p <= apply_rh) return p;
+  return p + (p > apply_rh + 4 * window ? 16u : 8u);
+}
+
 // FindLongestMatch (hash_longest_match64_inc.h:157, hash_longest_match_inc.h:156), lane-parallel:
 // every candidate's full match length is computed by its own lane, then the reference's
 // sequential "better than the best so far" rule is replayed with ballots.  The reference's
@@ -297,7 +326,7 @@ BR_DEV u32 br_ring_heavy(BrWalk& w, u32 j, u32 lo) {
 // first) -- with one match-length computation and one fold; further ring rows (32 entries each) follow from j - 28.
 template <int G>
 BR_DEV void br_find_longest_match(BrWalk& w, u32 cur, u32 max_length, u32 max_backward,
-                                  u32 dict_distance, BrSR& out) {
+                                  u32 dict_distance, BrSR& out, BrLook look = {~0u, 0u, 0u}) {
   const BrStream& s = *w.s;
   const BrParams& P = s.P;
   const u8* d = w.d;
@@ -337,6 +366,21 @@ BR_DEV void br_find_longest_match(BrWalk& w, u32 cur, u32 max_length, u32 max_ba
     // slot's candidate position; its first 8 bytes (distance cache); valid / has; the word of the S-ordered snapshot bits
     // that holds the entry's bit (ring)
     u32 ca[NC]; u64 ca0[NC]; bool cv[NC]; u32 csw[NC];
+#if BR_GPU && BR_WALK1_LOOKAHEAD > 0
+    // lookahead loads, requested with this search's own first round trip (the ranks share its sectors)
+    const u32 lrk = (u32)(lane - NDC);   // lane's row entry (lanes >= NDC)
+    // (a position is searched only while it lies more than htl bytes before the block end: rank exists there)
+    u32 jf[BR_WALK1_LOOKAHEAD];
+#pragma unroll
+    for (int i = 0; i < BR_WALK1_LOOKAHEAD; ++i) {
+      const u32 t = look.f0 + (u32)i;
+      jf[i] = (u32)i < look.nf && t < w.pend && w.pend - t > P.htl ? br_ldg(s.rank + t) : 0u;
+    }
+#if BR_WALK1_LOOKAHEAD >= 2
+    const u32 jn = look.next < w.pend && w.pend - look.next > P.htl ? br_ldg(s.rank + look.next) : 0u;
+    const u32 qn = lane >= NDC && lrk < block_size && jn > lrk ? br_ldg(s.S + (jn - 1 - lrk)) : 0u;
+#endif
+#endif
 #pragma unroll
     for (int i = 0; i < NC; ++i) {
       const int k = i * BR_WARP + lane;
@@ -360,6 +404,20 @@ BR_DEV void br_find_longest_match(BrWalk& w, u32 cur, u32 max_length, u32 max_ba
         ca0[i] = 0;
       }
     }
+#if BR_GPU && BR_WALK1_LOOKAHEAD > 0
+    // stage 1: the rows of S and their snapshot words, each lane its own entry (the row is one or two lines)
+#pragma unroll
+    for (int i = 0; i < BR_WALK1_LOOKAHEAD; ++i) {
+      if (lane >= NDC && jf[i] > lrk) {
+        br_prefetch_l2(s.S + (jf[i] - 1 - lrk));
+        br_prefetch_l2(s.storedS + ((jf[i] - 1 - lrk) >> 5));
+      }
+    }
+#if BR_WALK1_LOOKAHEAD >= 2
+    // stage 2: the first bytes of the next search's candidates
+    if (qn != 0 && qn < look.next && look.next - qn <= max_backward) br_prefetch_l2(d + qn);
+#endif
+#endif
     if (hi - lo >= P.heavy_min) V = br_ring_heavy(w, j, lo);
     br_own_sync(w);
     BR_W(8, 1); BR_W(1, 1);
@@ -861,7 +919,26 @@ BR_DEV void br_walk_one(const BrStream& s, u32 b, const BrBlockIn& in, BrBlockOu
       if constexpr (G == 0) {   // qualities 2..4 (k_walk<0>): best_len_in of the lazy search, backward_references_inc.h:127
         if (have) cur.len = br_min(sr.len - 1u, max_length);
         br_find_quick(w, sp, max_length, md, dd, cur);
-      } else br_find_longest_match<G>(w, sp, max_length, md, dd, cur);
+      } else {
+        BrLook look = {~0u, 0u, 0u};
+#if BR_GPU && BR_WALK1_LOOKAHEAD > 0
+        if (G == 1) {   // (the search uses it in the shared pass of quality 5 only)
+          if (have) {
+            // a lazy search: predicted to lose, so the parse goes on at position + sr.len.  That row was not prefetched
+            // (sr.len was not known), so only stage 1 runs for it and the positions behind it: loading it here for stage 2
+            // would put a round trip to HBM on this search.
+            look.f0 = position + sr.len; look.nf = BR_WALK1_LOOKAHEAD;
+          } else {
+            // predicted to fail (the parse goes on one position later, or jumps in a literal spree)
+            u32 n = br_next_search(sp, apply_random_heuristics, window);
+            if (BR_WALK1_LOOKAHEAD >= 2) look.next = n;
+            for (int i = 1; i < BR_WALK1_LOOKAHEAD; ++i) n = br_next_search(n, apply_random_heuristics, window);
+            look.f0 = n; look.nf = 1;
+          }
+        }
+#endif
+        br_find_longest_match<G>(w, sp, max_length, md, dd, cur, look);
+      }
       if (!have) {
         sr = cur;
         if (!(sr.score > BR_MIN_SCORE)) break;

@@ -33,7 +33,7 @@ BR_DEV void br_probe_search(const BrStream& s, u32* own, const u32* pr, u32* res
   const u32 cur = pr[0];
   BrSR sr; sr.len = pr[10]; sr.delta = 0; sr.distance = 0; sr.score = pr[11];
   if constexpr (G == 0) br_find_quick(w, cur, w.pend - cur, pr[4], pr[5], sr);
-  else br_find_longest_match<G>(w, cur, w.pend - cur, pr[4], pr[5], sr);
+  else br_find_longest_match<G>(w, cur, w.pend - cur, pr[4], pr[5], sr, BrLook{cur + 1, cur + 2, 1});   // (with a lookahead, which must not change the result)
   if (br_lane() == 0) {
     const bool here = w.acc_wi == (cur >> 5);
     res[0] = sr.len; res[1] = sr.distance; res[2] = sr.score; res[3] = (u32)sr.delta;
