@@ -587,8 +587,9 @@ static size_t scan_tmp_words(size_t n) { return n / SCAN_CHUNK + n / SCAN_CHUNK 
 // compressed bytes are left in device memory (*d_out, *out_size; valid until the next call on
 // this job).  Returns 1 on success, 0 on failure (unsupported parameters, CUDA error).
 // `cuts` (nullable): the stream is cut by FLUSH / EMIT_METADATA operations (br_pipeline.h BrCuts).
-extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 size_hint,
-                                      const u8* d_in, u32 n, const u8** d_out, size_t* out_size, const BrCuts* cuts) {
+// knobs (nullable): the schedule of the test hook br_debug_compress_sched.
+static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const u8* d_in, u32 n, const u8** d_out, size_t* out_size,
+                        const BrCuts* cuts, const BrSchedKnobs* knobs) {
   BrDeviceTables* T = get_tables();
   if (!T || n == 0) return 0;
   BrStream s; memset(&s, 0, sizeof(s));
@@ -605,6 +606,17 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
 #else
   const bool trace = false;
 #endif
+  if (knobs) {
+    if (knobs->sweep_epoch != BR_KNOB_KEEP) P.sweep_epoch = knobs->sweep_epoch;
+    if (knobs->force_epoch != BR_KNOB_KEEP) P.force_epoch = knobs->force_epoch;
+    if (knobs->step_cap != BR_KNOB_KEEP) P.step_cap = knobs->step_cap;
+    if (knobs->heavy_min != BR_KNOB_KEEP) P.heavy_min = knobs->heavy_min;
+    if (knobs->pilot != BR_KNOB_KEEP) P.pilot = knobs->pilot;
+    if (knobs->sweep_blocks != BR_KNOB_KEEP) {
+      if (knobs->sweep_blocks == 0 || (knobs->sweep_blocks & (knobs->sweep_blocks - 1))) return 0;   // (a power of two)
+      P.sweep_blocks = knobs->sweep_blocks;
+    }
+  }
   // chunk / block tables: the reference's input blocks (1 << lgblock bytes, shorter where a FLUSH cut the input)
   std::vector<BrBlk> hblk;
   const u32 ncuts = cuts ? cuts->n : 0;
@@ -674,7 +686,11 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
   int* changed_epoch = A.take<int>(nb + 16); u32* ext_total = A.take<u32>(nb + 16);
   u32* cmd_off = A.take<u32>(nb + 16); u32* force_unc = A.take<u32>(nb + 16);
   u32* dirty_list = A.take<u32>(nb + 16); u32* block_mb = A.take<u32>(nb + 16);
+  // ran_list: every chunk is walked at most once per launch -- by its own scheduled walker or by the one sweep that chases
+  // into it, and in a forced launch the walkers scheduled behind the forced one in its input block stand down
+  // (br_walk_block) -- so a launch appends at most nb entries
   u32* ran_list = A.take<u32>(nb + 16); u32* lil_in = A.take<u32>(nb + 16);
+  job->stats.ran_cap = nb + 16;
   int* bitdep_epoch = A.take<int>(nb + 16);
   BrBlk* d_blk = A.take<BrBlk>(nblk); BrBlkIn* d_blkin = A.take<BrBlkIn>(nblk);
   u32* key_flips = A.take<u32>(P.nbuckets + 8);
@@ -777,6 +793,7 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
       CK(cudaStreamSynchronize(st));
       u32 n_dirty = hp[0], n_sched = hp[5]; n_mbs = hp[1]; total_cmds = hp[2];
       job->stats.block_runs += hp[4];
+      if (hp[4] > job->stats.max_walks) job->stats.max_walks = hp[4];
       if (trace) fprintf(stderr, "epoch %u: dirty %u sched %u ran %u longest sweep %u | never %u state %u dict %u bits %u wrap %u\n", s.epoch, hp[0], hp[5], hp[4], hp[16], hp[9], hp[10], hp[11], hp[12], hp[13]);
       if (walk_pending) {
         float wms; cudaEventElapsedTime(&wms, ev[6], ev[7]); job->stats.ms_walk += wms; walk_pending = false;
@@ -786,6 +803,7 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
       if (s.epoch + 2 >= P.max_epochs) { fprintf(stderr, "brotli_b200: internal error: launch bound exceeded\n"); return 0; }
       ++s.epoch; ++job->stats.lz77_iterations;
       s.forced = s.epoch - round_epoch0 >= P.force_epoch ? 1u : 0u;
+      job->stats.forced_launches += s.forced;
       CK(cudaMemsetAsync(bits_cur, 0, 2 * (size_t)nwords * 4, st));
       CK(cudaMemsetAsync(srch_cur, 0, nwords * 4, st));
       CK(cudaMemsetAsync(counters + 4, 0, 4, st));
@@ -933,6 +951,37 @@ extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 si
   }
   *d_out = final_out; *out_size = final_size;
   return 1;
+}
+
+extern "C" int br_job_compress_device(BrJob* job, int quality, int lgwin, u32 size_hint,
+                                      const u8* d_in, u32 n, const u8** d_out, size_t* out_size, const BrCuts* cuts) {
+  return job_compress(job, quality, lgwin, size_hint, d_in, n, d_out, out_size, cuts, nullptr);
+}
+
+// Test hook (tests/test_zz_gpu_schedule.py): one stream through br_job_compress_device with the fixpoint's schedule knobs
+// set on the host (BrSchedKnobs).  stats (8 words): launches, chunk walks, chunks, forced launches, the most walks of one
+// launch, ran_list capacity, rounds.  Returns the compressed size, 0 on failure, -1 when it does not fit out_cap.
+extern "C" __attribute__((visibility("default"))) long br_debug_compress_sched(int quality, int lgwin, const u8* h_in, u32 n,
+                                                                              const BrSchedKnobs* knobs, u8* h_out, size_t out_cap,
+                                                                              u32* stats) {
+  if (n == 0 || !knobs) return 0;
+  BrJob* job = br_job_create();
+  if (!job) return 0;
+  long ret = 0;
+  u8* d_in = nullptr;
+  const u8* d_out = nullptr; size_t sz = 0;
+  if (cudaMalloc(&d_in, n) == cudaSuccess && cudaMemcpy(d_in, h_in, n, cudaMemcpyHostToDevice) == cudaSuccess &&
+      job_compress(job, quality, lgwin, n, d_in, n, &d_out, &sz, nullptr, knobs)) {
+    if (sz > out_cap) ret = -1;
+    else if (cudaMemcpy(h_out, d_out, sz, cudaMemcpyDeviceToHost) == cudaSuccess) ret = (long)sz;
+    const BrJobStats& t = job->stats;
+    const u32 v[8] = {t.lz77_iterations, (u32)t.block_runs, t.nblocks, t.forced_launches, t.max_walks, t.ran_cap, t.rounds, 0};
+    memcpy(stats, v, sizeof(v));
+  }
+  cudaGetLastError();
+  if (d_in) cudaFree(d_in);
+  br_job_destroy(job);
+  return ret;
 }
 
 // Debug / test hooks: the position index of a one-stream job, built by br_build_index and copied to the host.

@@ -26,6 +26,7 @@ struct BrSR { u32 len, distance, score; int delta; };
 #ifdef BR_SIM_DEBUG
 static u64 br_sim_w[12];   // tests/sim: 0 searches, 1 ring rows, 2 heavy-path searches, 3 heavy own-scan rows, 4 countS calls, 5 own_set, 6 set_range, 7 dict searches, 8 ring groups, 9 candidates taken, 10 match_len beyond 16 bytes
 #define BR_W(i, n) (br_sim_w[i] += (n))
+static u64 br_sim_bnd[2];  // tests/sim: block boundaries a sweep reached where br_predict_next_block 0 accepted, 1 refused
 #else
 #define BR_W(i, n)
 #endif
@@ -1081,8 +1082,16 @@ BR_DEV bool br_predict_next_block(const BrStream& s, u32 b, const BrBlockIn& in,
 // the sequential parse of that stretch: serial ripples (the position phase of the sparse search running through
 // incompressible data, a distance-cache change flowing through match-free data) cost one launch per input block, not
 // one launch per chunk.
+//
+// A forced launch (BrStream::forced): the walker of the first scheduled chunk runs to the end of its input block
+// (`to_block_end`) through every chunk behind it, so the walkers scheduled behind it in that block stand down.  Were they to
+// walk too, those chunks would be walked twice in one launch by walkers that share one chunk record (bout, bin_used,
+// cmd_blocks) and, at equal head parity, one bits_cur bitmap: each walk would read the other's fresh stored-bits as its own,
+// the commit would store their union, and the fixpoint could settle on bits no walk of the chunk produced (DESIGN.md
+// section 3).  So every chunk is walked at most once per launch, and a launch appends at most nblocks entries to ran_list.
 template <int G, bool M = false>
 BR_DEV void br_walk_block(const BrStream& s, u32 b, bool to_block_end) {
+  if (s.forced && !to_block_end && s.bin[b].blk == s.bin[s.counters[6]].blk) return;
   BrBlockIn in = s.bin[b];
   const u32 head = b;
   u32 sweep_p0 = 0xffffffffu;
@@ -1096,7 +1105,11 @@ BR_DEV void br_walk_block(const BrStream& s, u32 b, bool to_block_end) {
       // block boundary: crossed by the sweeps of a sweep-mode launch, inside a group of sweep_blocks blocks
       const bool full_sweep = s.epoch > s.P.sweep_epoch + 9 && (s.epoch - 1 - s.P.sweep_epoch) % 3 == 0;   // (as br_chain_c decided it)
       if (to_block_end || in.is_last || nb >= s.P.nblocks || s.epoch <= s.P.sweep_epoch || full_sweep || ((in.blk + 1) & (s.P.sweep_blocks - 1u)) == 0) return;
-      if (!br_predict_next_block(s, b, in, o, ni)) return;
+      const bool crossed = br_predict_next_block(s, b, in, o, ni);
+#ifdef BR_SIM_DEBUG
+      ++br_sim_bnd[crossed ? 0 : 1];
+#endif
+      if (!crossed) return;
     } else {
       ni = s.bin[nb];
       ni.start_pos = o.out_pos; ni.apply_rh = o.apply_rh; ni.store_end = o.store_end; ni.ext_dist = 0; ni.warm = 0;

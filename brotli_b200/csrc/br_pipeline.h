@@ -10,7 +10,14 @@ struct BrJobStats {
   uint64_t walk_bytes, total_cmds;   // input bytes walked (all launches), commands emitted
   uint32_t lz77_iterations, nblocks, n_metablocks, rounds, launches;
   uint64_t block_runs, in_bytes, out_bytes;
+  uint32_t forced_launches;          // walk launches with a forced walker (BrParams::force_epoch)
+  uint32_t max_walks, ran_cap;       // the most chunk walks of one launch, and how many ran_list holds
 };
+// The schedule knobs of the LZ77 fixpoint (BrParams: sweep_epoch, force_epoch, step_cap, heavy_min, pilot, sweep_blocks) for
+// the test hook br_debug_compress_sched; BR_KNOB_KEEP keeps the value br_derive_params chose.  The bytes must not depend on
+// them: every legal schedule ends on the sequential parse.
+#define BR_KNOB_KEEP 0xffffffffu
+struct BrSchedKnobs { uint32_t sweep_epoch, force_epoch, step_cap, heavy_min, pilot, sweep_blocks; };
 // A stream cut by FLUSH / EMIT_METADATA operations (c/enc/encode.c:1634): pos[i] (sorted, in (0, n]) = input position where
 // the i-th such operation ended the input, kind[i] = 1 FLUSH, 2 EMIT_METADATA.  is_final = 0: FINISH has not been seen, the
 // stream ends behind the cut at n.  with_header = 0: the window bits were already sent.  end_bit (host, nullable) receives
@@ -32,6 +39,8 @@ void* br_job_stream(BrJob*);
 int br_job_compress_device(BrJob* job, int quality, int lgwin, uint32_t size_hint,
                            const uint8_t* d_in, uint32_t n, const uint8_t** d_out, size_t* out_size, const BrCuts* cuts);
 int br_debug_sort(int quality, int lgwin, const uint8_t* h_in, uint32_t n, uint32_t* h_S, uint32_t* h_seg);
+long br_debug_compress_sched(int quality, int lgwin, const uint8_t* h_in, uint32_t n, const BrSchedKnobs* knobs, uint8_t* h_out,
+                            size_t out_cap, uint32_t* stats);
 int br_debug_index(int quality, int lgwin, const uint8_t* h_in, uint32_t n, uint32_t* h_S, uint32_t* h_seg, uint32_t* h_rank,
                    uint32_t* h_keys);
 }

@@ -34,6 +34,34 @@ extern "C" int sim_init(const u8* blob, size_t len, u32 log2n) {
   return 1;
 }
 
+// An explicit schedule of the LZ77 fixpoint (sim_compress_sched): the knobs of BrParams that decide which chunks a launch
+// walks and when the safety nets take over, and the order in which the sim runs a launch's walks and commits (on the GPU
+// they run concurrently, in no fixed order).  SIM_KEEP keeps the value br_derive_params chose.
+#define SIM_KEEP 0xffffffffu
+enum { SIM_ORDER_SCHEDULED = 0, SIM_ORDER_REVERSED = 1, SIM_ORDER_SHUFFLED = 2 };
+struct SimSched {
+  u32 sweep_epoch, force_epoch, step_cap, heavy_min, pilot, sweep_blocks;
+  u32 batch_chunk_bits;             // chunk size of a batch of streams (log2)
+  u32 walk_order, commit_order;     // SIM_ORDER_*; commit_order applies to the br_cover_run and the br_commit_bits loops
+  u32 walk_seed, commit_seed;       // SIM_ORDER_SHUFFLED
+  u32 verify;                       // != 0: re-walk every chunk at the fixpoint (SIM_ST_VERIFY_DIFF); the output is unchanged
+};
+// stats words of sim_compress_sched (the first five as sim_compress reports them)
+enum {
+  SIM_ST_LAUNCHES = 0, SIM_ST_WALKS = 1, SIM_ST_CHUNKS = 2, SIM_ST_ROUNDS = 3, SIM_ST_MODEL_COST = 4,
+  SIM_ST_FULL_SWEEP = 5,        // launches that follow a full-sweep chain decision (br_chain_c)
+  SIM_ST_FORCED = 6,            // launches with a forced walker (BrStream::forced)
+  SIM_ST_STEP_CAP = 7,          // step-cap hits of br_commit_bits (BR_SIM_DEBUG builds only)
+  SIM_ST_PREDICT_OK = 8,        // block boundaries a sweep crossed (br_predict_next_block true; BR_SIM_DEBUG builds only)
+  SIM_ST_PREDICT_NO = 9,        // block boundaries where the prediction refused (BR_SIM_DEBUG builds only)
+  SIM_ST_MAX_WALKS = 10,        // the largest number of chunk walks of one launch (counters[4])
+  SIM_ST_RAN_CAP = 11,          // capacity of ran_list, as the product sizes it
+  SIM_ST_VERIFY_DIFF = 12,      // chunks whose re-walk at the fixpoint gives other bits or another out-state (SimSched::verify)
+  SIM_ST_WORDS = 16
+};
+#define SIM_ERR_CAPACITY (-5)   // a launch appended more entries than an array holds (the call fails, nothing is corrupted)
+#define SIM_ERR_NO_FIXPOINT (-6)   // the launch bound (BrParams::max_epochs) was reached
+
 struct SimStream {
   BrStream s;
   std::vector<u8> data;
@@ -53,6 +81,9 @@ struct SimStream {
   int iterations = 0;
   u64 block_runs = 0;
   double model_cost = 0;
+  SimSched sched;
+  u32 ran_cap = 0;
+  u32 st[SIM_ST_WORDS] = {};
 };
 
 static void sim_build_sorted(SimStream& m) {
@@ -88,7 +119,19 @@ static void sim_build_storedS(SimStream& m) {
 }
 
 struct SimCuts { const u32* pos; const u32* kind; u32 n; int is_final; int with_header; int finish_empty; u64* end_bit; u32 size_hint; int lgblock; int disable_ctx; u32 stream_offset; u64* stream_end; };
-static SimStream* sim_setup(int q, int lgwin, const u8* in, u32 n, const SimCuts* cuts = nullptr) {
+// the schedule of the tools' environment switches (BR_SIM_*): everything else as derived, walks and commits in list order
+static SimSched sim_sched_from_env() {
+  SimSched c;
+  auto env = [](const char* name) { const char* v = getenv(name); return v ? (u32)atoi(v) : SIM_KEEP; };
+  c.heavy_min = env("BR_SIM_HEAVY_MIN"); c.step_cap = env("BR_SIM_STEP_CAP"); c.sweep_epoch = env("BR_SIM_SWEEP_EPOCH");
+  c.sweep_blocks = env("BR_SIM_SWEEP_BLOCKS"); c.pilot = env("BR_SIM_PILOT"); c.force_epoch = env("BR_SIM_FORCE_EPOCH");
+  c.batch_chunk_bits = env("BR_SIM_BATCH_CHUNK_BITS");
+  c.walk_order = c.commit_order = SIM_ORDER_SCHEDULED; c.walk_seed = c.commit_seed = 0;
+  c.verify = getenv("BR_SIM_VERIFY") ? 1u : 0u;
+  return c;
+}
+
+static SimStream* sim_setup(int q, int lgwin, const u8* in, u32 n, const SimCuts* cuts = nullptr, const SimSched* sched = nullptr) {
   SimStream* m = new SimStream();
   BrStream& s = m->s;
   memset(&s, 0, sizeof(s));
@@ -96,14 +139,16 @@ static SimStream* sim_setup(int q, int lgwin, const u8* in, u32 n, const SimCuts
   s.P.disable_ctx = cuts && cuts->disable_ctx ? 1u : 0u;
   s.P.stream_offset = cuts ? (cuts->stream_offset < s.P.max_backward ? cuts->stream_offset : s.P.max_backward) : 0u;
   BrParams& P = s.P;
-  if (getenv("BR_SIM_HEAVY_MIN")) P.heavy_min = (u32)atoi(getenv("BR_SIM_HEAVY_MIN"));
-  if (getenv("BR_SIM_STEP_CAP")) P.step_cap = (u32)atoi(getenv("BR_SIM_STEP_CAP"));
-  if (getenv("BR_SIM_SWEEP_EPOCH")) P.sweep_epoch = (u32)atoi(getenv("BR_SIM_SWEEP_EPOCH"));
-  if (getenv("BR_SIM_SWEEP_BLOCKS")) P.sweep_blocks = (u32)atoi(getenv("BR_SIM_SWEEP_BLOCKS"));
-  if (getenv("BR_SIM_PILOT")) P.pilot = (u32)atoi(getenv("BR_SIM_PILOT"));
-  if (getenv("BR_SIM_FORCE_EPOCH")) P.force_epoch = (u32)atoi(getenv("BR_SIM_FORCE_EPOCH"));
+  m->sched = sched ? *sched : sim_sched_from_env();
+  const SimSched& K = m->sched;
+  if (K.heavy_min != SIM_KEEP) P.heavy_min = K.heavy_min;
+  if (K.step_cap != SIM_KEEP) P.step_cap = K.step_cap;
+  if (K.sweep_epoch != SIM_KEEP) P.sweep_epoch = K.sweep_epoch;
+  if (K.sweep_blocks != SIM_KEEP) P.sweep_blocks = K.sweep_blocks;
+  if (K.pilot != SIM_KEEP) P.pilot = K.pilot;
+  if (K.force_epoch != SIM_KEEP) P.force_epoch = K.force_epoch;
   { u32 ns = 1; for (u32 i = 0; cuts && i < cuts->n; ++i) if (cuts->kind[i] == 3) ++ns;
-    if (ns > 1) { P.pilot = 0; P.multi = ns; P.chunk_bits = getenv("BR_SIM_BATCH_CHUNK_BITS") ? (u32)atoi(getenv("BR_SIM_BATCH_CHUNK_BITS")) : br_batch_chunk_bits(n); } }   // (as br_job_compress_device)
+    if (ns > 1) { P.pilot = 0; P.multi = ns; P.chunk_bits = K.batch_chunk_bits != SIM_KEEP ? K.batch_chunk_bits : br_batch_chunk_bits(n); } }   // (as br_job_compress_device)
   const u32 ch = 1u << P.chunk_bits;
   std::vector<BrBlockIn> chunks;
   P.finish_empty = cuts && cuts->finish_empty ? 1u : 0u;
@@ -140,7 +185,7 @@ static SimStream* sim_setup(int q, int lgwin, const u8* in, u32 n, const SimCuts
     s.stream_blk = m->stream_blk.data(); s.stream_nmb = m->stream_nmb.data(); s.stream_ncmd = m->stream_ncmd.data(); s.mbs_stage = m->mbs_stage.data();
   }
   s.cmd_stride = ch / 2 + 2;
-  m->cmd_blocks.resize((size_t)nb * s.cmd_stride);
+  m->cmd_blocks.resize((size_t)(nb + 1) * s.cmd_stride);   // (+ a guard slice behind the last chunk's: see sim_lz77_fixpoint)
   s.bits_latest = m->bits_latest.data(); s.bits_cur = m->bits_cur.data(); s.bits_words = (u32)m->bits_latest.size();
   s.srch_latest = m->srch_latest.data(); s.srch_cur = m->srch_cur.data(); s.cover_cur = m->cover_cur.data();
   s.storedS = m->storedS.data(); s.prefS = m->prefS.data();
@@ -157,7 +202,10 @@ static SimStream* sim_setup(int q, int lgwin, const u8* in, u32 n, const SimCuts
   if (P.quick) { m->saw.assign(((size_t)n << P.qk_sweep_bits) + 4, 0xdeadbeefu); s.saw = m->saw.data(); }
   m->dirty_list.assign(nb + 1, 0); m->block_mb.assign(nb + 1, 0);
   s.dirty_list = m->dirty_list.data(); s.block_mb = m->block_mb.data();
-  m->ran_list.assign(nb + 1, 0); s.ran_list = m->ran_list.data();
+  // ran_list as the product sizes it (br_job_compress_device), followed by a guard as long again: a launch that appends
+  // more walks than the product holds writes into the guard, and the fixpoint fails the call (SIM_ERR_CAPACITY)
+  m->ran_cap = nb + 16;
+  m->ran_list.assign(2 * (size_t)m->ran_cap, 0); s.ran_list = m->ran_list.data();
   const u8* p = g_t.blob.data() + 8;
   s.dict_size_bits = p; p += 32;
   s.dict_offsets = (const u32*)p; p += 128;
@@ -175,11 +223,33 @@ static SimStream* sim_setup(int q, int lgwin, const u8* in, u32 n, const SimCuts
   return m;
 }
 
-static void sim_lz77_fixpoint(SimStream& m) {
+// The order in which the sim runs the n entries of a launch's list (SimSched::walk_order / commit_order).  The shuffle is a
+// Fisher-Yates draw from a 64-bit LCG seeded by (seed, launch, pass): reproducible on every platform.
+static std::vector<u32> sim_order(u32 n, u32 order, u32 seed, u32 launch, u32 pass) {
+  std::vector<u32> o(n);
+  for (u32 i = 0; i < n; ++i) o[i] = order == SIM_ORDER_REVERSED ? n - 1 - i : i;
+  if (order == SIM_ORDER_SHUFFLED) {
+    u64 x = ((u64)seed << 32) ^ ((u64)launch << 8) ^ pass ^ 0x9E3779B97F4A7C15ull;
+    for (u32 i = n; i > 1; --i) {
+      x = x * 6364136223846793005ull + 1442695040888963407ull;
+      std::swap(o[i - 1], o[(u32)((x >> 33) % i)]);
+    }
+  }
+  return o;
+}
+
+// Is the fixpoint self-consistent?  Re-walks every chunk from its final in-state against the final stored-bits and returns
+// the number of chunks whose bits or out-state come out differently.  Everything the re-walk writes is restored afterwards,
+// so the output is that of the fixpoint.
+static u32 sim_verify_fixpoint(SimStream& m);
+
+// Runs the LZ77 fixpoint; 0, or SIM_ERR_CAPACITY when a launch appended more entries than an array of the product holds.
+static int sim_lz77_fixpoint(SimStream& m) {
   BrStream& s = m.s; u32 nb = s.P.nblocks;
 #ifdef BR_SIM_DEBUG
   if (getenv("BR_SIM_WATCH")) br_sim_watch = (u32)atoi(getenv("BR_SIM_WATCH"));
 #endif
+  const SimSched& K = m.sched;
   // (the launch counter runs on through the rounds of a late fallback, as in br_job_compress_device: runs are stamped with
   // it -- BrBlockOut::epoch -- and the marks of br_commit_bits / br_verify_run are compared with those stamps)
   const u32 round_epoch0 = s.epoch;
@@ -194,16 +264,30 @@ static void sim_lz77_fixpoint(SimStream& m) {
 #endif
     }
     if (s.counters[0] == 0) break;
+    // (the rule of br_chain_c, at the launch number the chain ran with)
+    if (s.epoch >= s.P.sweep_epoch + 9 && (s.epoch - s.P.sweep_epoch) % 3 == 0) ++m.st[SIM_ST_FULL_SWEEP];
     ++s.epoch; ++m.iterations;
     sim_build_storedS(m);
     std::fill(m.bits_cur.begin(), m.bits_cur.end(), 0); std::fill(m.srch_cur.begin(), m.srch_cur.end(), 0);
     s.counters[4] = 0; s.counters[16] = 0;
     s.forced = s.epoch - round_epoch0 >= s.P.force_epoch;
-    { u32 nd = s.counters[5]; std::vector<u32> dl(nd); for (u32 t = 0; t < nd; ++t) dl[t] = br_sched_entry(s, t); for (u32 k : dl) { const bool f = s.forced && k == s.counters[6];
+    if (s.forced) ++m.st[SIM_ST_FORCED];
+    { u32 nd = s.counters[5]; std::vector<u32> dl(nd); for (u32 t = 0; t < nd; ++t) dl[t] = br_sched_entry(s, t);
+      for (u32 t : sim_order(nd, K.walk_order, K.walk_seed, s.epoch, 0)) { const u32 k = dl[t]; const bool f = s.forced && k == s.counters[6];
       if (s.P.quick) { if (s.P.multi) br_walk_block<0, true>(s, k, f); else br_walk_block<0>(s, k, f); }
       else if (s.P.multi) { if (s.P.block_bits >= 6) br_walk_block<4, true>(s, k, f); else br_walk_block<1, true>(s, k, f); }
       else if (s.P.block_bits >= 6) br_walk_block<4>(s, k, f); else br_walk_block<1>(s, k, f); } }
     m.block_runs += s.counters[4];
+    if (s.counters[4] > m.st[SIM_ST_MAX_WALKS]) m.st[SIM_ST_MAX_WALKS] = s.counters[4];
+    if (s.counters[4] > m.ran_cap) {
+      fprintf(stderr, "sim: launch %u walked %u chunks, ran_list holds %u\n", s.epoch, s.counters[4], m.ran_cap);
+      return SIM_ERR_CAPACITY;
+    }
+    for (u32 i = 0; i < s.counters[4]; ++i)
+      if (s.bout[s.ran_list[i]].ncmd > s.cmd_stride) {
+        fprintf(stderr, "sim: chunk %u made %u commands, its slice of cmd_blocks holds %u\n", s.ran_list[i], s.bout[s.ran_list[i]].ncmd, s.cmd_stride);
+        return SIM_ERR_CAPACITY;
+      }
 #ifdef BR_SIM_DEBUG
     if (getenv("BR_SIM_TRACE")) { fprintf(stderr, "   work: searches %llu rows %llu groups %llu taken %llu | heavy %llu own-scan rows %llu countS %llu | own_set %llu set_range %llu dict %llu\n",
       (unsigned long long)br_sim_w[0], (unsigned long long)br_sim_w[1], (unsigned long long)br_sim_w[8], (unsigned long long)br_sim_w[9], (unsigned long long)br_sim_w[2], (unsigned long long)br_sim_w[3],
@@ -216,59 +300,94 @@ static void sim_lz77_fixpoint(SimStream& m) {
     }
     m.bits_prev = m.bits_latest; s.bits_prev = m.bits_prev.data();
     std::fill(m.cover_cur.begin(), m.cover_cur.end(), 0);
-    for (u32 i = 0; i < s.counters[4]; ++i) br_cover_run(s, s.ran_list[i]);
-    for (u32 i = 0; i < s.counters[4]; ++i) br_commit_bits(s, s.ran_list[i]);
+    // (every run is covered before any commit, as k_cover runs before k_commit on the GPU)
+    for (u32 i : sim_order(s.counters[4], K.commit_order, K.commit_seed, s.epoch, 1)) br_cover_run(s, s.ran_list[i]);
+#ifdef BR_SIM_DEBUG
+    const u64 cap_hits0 = br_sim_cnt[2];
+#endif
+    for (u32 i : sim_order(s.counters[4], K.commit_order, K.commit_seed, s.epoch, 2)) br_commit_bits(s, s.ran_list[i]);
+#ifdef BR_SIM_DEBUG
+    m.st[SIM_ST_STEP_CAP] += (u32)(br_sim_cnt[2] - cap_hits0);
+#endif
     if (s.P.quick) for (u32 k = 0; k < nb; ++k) br_verify_run(s, k);
-    if (s.epoch + 2 >= s.P.max_epochs) { fprintf(stderr, "sim: no fixpoint\n"); break; }
+    if (s.epoch + 2 >= s.P.max_epochs) { fprintf(stderr, "sim: no fixpoint\n"); return SIM_ERR_NO_FIXPOINT; }
   }
+  if (K.verify) m.st[SIM_ST_VERIFY_DIFF] += sim_verify_fixpoint(m);
   if (getenv("BR_SIM_TRACE")) {   // the static-dictionary gate (hash.h:186) at the fixpoint: chunks that start with it closed
     u32 closed = 0, hits = 0; for (u32 k = 0; k < nb; ++k) { const u64 l = ((u64)s.bin[k].dict_l_hi << 32) | s.bin[k].dict_l_lo, mm = ((u64)s.bin[k].dict_m_hi << 32) | s.bin[k].dict_m_lo; if (mm < (l >> 7)) ++closed; if (s.bout[k].dm) ++hits; }
     fprintf(stderr, "dictionary gate: %u of %u chunks start with the gate closed; %u chunks found dictionary matches\n", closed, nb, hits);
   }
-  if (getenv("BR_SIM_VERIFY")) {
-    // Is the fixpoint self-consistent?  Re-walk every chunk from its final in-state against the final
-    // stored-bits and report the chunks whose bits or out-state come out differently.
-    ++s.epoch;
-    std::fill(m.bits_cur.begin(), m.bits_cur.end(), 0); std::fill(m.srch_cur.begin(), m.srch_cur.end(), 0);
-    std::vector<BrBlockOut> old(s.bout, s.bout + nb);
-    std::vector<BrCmd> old_cmds(m.cmd_blocks);
-    s.counters[4] = 0;
-    for (u32 k = 0; k < nb; ++k) { BrBlockOut o; u32 sp0 = 0xffffffffu; if (s.P.quick && s.P.multi) br_walk_one<0, true>(s, k, s.bin[k], o, k, sp0); else if (s.P.quick) br_walk_one<0>(s, k, s.bin[k], o, k, sp0); else br_walk_one<1>(s, k, s.bin[k], o, k, sp0); }
-    m.bits_prev = m.bits_latest; s.bits_prev = m.bits_prev.data();
-    std::fill(m.cover_cur.begin(), m.cover_cur.end(), 0);
-    for (u32 k = 0; k < nb; ++k) br_cover_run(s, k);
-    for (u32 k = 0; k < nb; ++k) {
-      br_commit_bits(s, k);
-      const BrBlockOut& a = old[k]; const BrBlockOut& b = s.bout[k];
-      bool same = a.ncmd == b.ncmd && a.nlit == b.nlit && a.out_pos == b.out_pos && a.last_insert_len == b.last_insert_len &&
-                  !memcmp(a.dc, b.dc, sizeof(a.dc)) && a.apply_rh == b.apply_rh;
-      if (s.changed_bits[k] && getenv("BR_SIM_VERIFY")[0] == '2') {
-        u32 shown = 0;
-        for (u32 q = s.bin_used[k].start_pos; q < s.bout[k].out_pos && shown < 12; ++q) {
-          u32 o = (m.bits_prev[q >> 5] >> (q & 31)) & 1, n2 = (m.bits_latest[q >> 5] >> (q & 31)) & 1;
-          if (o != n2) { fprintf(stderr, "  pos %u: fixpoint %u rewalk %u\n", q, o, n2); ++shown; }
-        }
-      }
-      if (!same || memcmp(&old_cmds[(size_t)k * s.cmd_stride], &m.cmd_blocks[(size_t)k * s.cmd_stride], (size_t)std::min(a.ncmd, b.ncmd) * sizeof(BrCmd))) {
-        // first command that differs: where it starts in the input, what it was and what the re-walk says
-        u32 pos = s.bin[k].start_pos;
-        for (u32 i = 0; i < std::min(a.ncmd, b.ncmd); ++i) {
-          const BrCmd& x = old_cmds[(size_t)k * s.cmd_stride + i]; const BrCmd& y = m.cmd_blocks[(size_t)k * s.cmd_stride + i];
-          if (memcmp(&x, &y, sizeof(BrCmd))) {
-            fprintf(stderr, "verify: chunk %u (run of launch %u) command %u at input %u: fixpoint insert %u copy %u dist_prefix %u extra %u | rewalk insert %u copy %u dist_prefix %u extra %u\n", k, a.epoch, i, pos,
-                    x.insert_len, x.copy_len & 0x1FFFFFF, x.dist_prefix, x.dist_extra, y.insert_len, y.copy_len & 0x1FFFFFF, y.dist_prefix, y.dist_extra);
-            break;
-          }
-          pos += x.insert_len + (x.copy_len & 0x1FFFFFF);
-        }
-      }
-      if (s.changed_bits[k] || !same)
-        fprintf(stderr, "verify: chunk %u [%u..%u) start %u: %u bits differ, out-state %s (ncmd %u/%u out_pos %u/%u)\n", k, s.bin[k].pos, s.bin[k].end,
-                s.bin[k].start_pos, s.changed_bits[k], same ? "same" : "DIFFERENT", a.ncmd, b.ncmd, a.out_pos, b.out_pos);
-    }
-  }
   m.cmds_all.resize(s.counters[2] + 1);
   for (u32 k = 0; k < nb; ++k) br_compact_block(s, k, m.cmds_all.data(), m.block_mb.data());
+  return 0;
+}
+
+static u32 sim_verify_fixpoint(SimStream& m) {
+  BrStream& s = m.s; const u32 nb = s.P.nblocks;
+  const char* show = getenv("BR_SIM_VERIFY");   // (the tools: print what differs; "2" also the positions)
+  // what the re-walk and its commits write
+  const u32 epoch0 = s.epoch;
+  const std::vector<BrBlockOut> old(m.bout);
+  const std::vector<BrBlockIn> used0(m.bin_used);
+  const std::vector<BrCmd> old_cmds(m.cmd_blocks);
+  const std::vector<u32> latest0(m.bits_latest), srch0(m.srch_latest), counters0(m.counters), key_flips0(m.key_flips), saw0(m.saw), changed_bits0(m.changed_bits);
+  const std::vector<int> bitdep0(m.bitdep_epoch), changed_epoch0(m.changed_epoch);
+  const std::vector<BrBlk> blks0(m.blks);
+  ++s.epoch;
+  sim_build_storedS(m);   // (the S-ordered snapshot of the final bits: the last launch's commits are not in it yet)
+  std::fill(m.bits_cur.begin(), m.bits_cur.end(), 0); std::fill(m.srch_cur.begin(), m.srch_cur.end(), 0);
+  s.counters[4] = 0;
+  for (u32 k = 0; k < nb; ++k) {
+    BrBlockOut o; u32 sp0 = 0xffffffffu;
+    if (s.P.quick) { if (s.P.multi) br_walk_one<0, true>(s, k, s.bin[k], o, k, sp0); else br_walk_one<0>(s, k, s.bin[k], o, k, sp0); }
+    else if (s.P.multi) { if (s.P.block_bits >= 6) br_walk_one<4, true>(s, k, s.bin[k], o, k, sp0); else br_walk_one<1, true>(s, k, s.bin[k], o, k, sp0); }
+    else if (s.P.block_bits >= 6) br_walk_one<4>(s, k, s.bin[k], o, k, sp0); else br_walk_one<1>(s, k, s.bin[k], o, k, sp0);
+  }
+  m.bits_prev = m.bits_latest; s.bits_prev = m.bits_prev.data();
+  std::fill(m.cover_cur.begin(), m.cover_cur.end(), 0);
+  for (u32 k = 0; k < nb; ++k) br_cover_run(s, k);
+  u32 ndiff = 0;
+  for (u32 k = 0; k < nb; ++k) {
+    br_commit_bits(s, k);
+    const BrBlockOut& a = old[k]; const BrBlockOut& b = s.bout[k];
+    const bool same = a.ncmd == b.ncmd && a.nlit == b.nlit && a.out_pos == b.out_pos && a.last_insert_len == b.last_insert_len &&
+                      !memcmp(a.dc, b.dc, sizeof(a.dc)) && a.apply_rh == b.apply_rh;
+    const bool same_cmds = same && !memcmp(&old_cmds[(size_t)k * s.cmd_stride], &m.cmd_blocks[(size_t)k * s.cmd_stride], (size_t)a.ncmd * sizeof(BrCmd));
+    if (s.changed_bits[k] || !same_cmds) ++ndiff;
+    if (!show) continue;
+    if (s.changed_bits[k] && show[0] == '2') {
+      u32 shown = 0;
+      for (u32 q = s.bin_used[k].start_pos; q < s.bout[k].out_pos && shown < 12; ++q) {
+        u32 o = (m.bits_prev[q >> 5] >> (q & 31)) & 1, n2 = (m.bits_latest[q >> 5] >> (q & 31)) & 1;
+        if (o != n2) { fprintf(stderr, "  pos %u: fixpoint %u rewalk %u\n", q, o, n2); ++shown; }
+      }
+    }
+    if (!same_cmds) {
+      // first command that differs: where it starts in the input, what it was and what the re-walk says
+      u32 pos = s.bin[k].start_pos;
+      for (u32 i = 0; i < std::min(a.ncmd, b.ncmd); ++i) {
+        const BrCmd& x = old_cmds[(size_t)k * s.cmd_stride + i]; const BrCmd& y = m.cmd_blocks[(size_t)k * s.cmd_stride + i];
+        if (memcmp(&x, &y, sizeof(BrCmd))) {
+          fprintf(stderr, "verify: chunk %u (run of launch %u) command %u at input %u: fixpoint insert %u copy %u dist_prefix %u extra %u | rewalk insert %u copy %u dist_prefix %u extra %u\n", k, a.epoch, i, pos,
+                  x.insert_len, x.copy_len & 0x1FFFFFF, x.dist_prefix, x.dist_extra, y.insert_len, y.copy_len & 0x1FFFFFF, y.dist_prefix, y.dist_extra);
+          break;
+        }
+        pos += x.insert_len + (x.copy_len & 0x1FFFFFF);
+      }
+    }
+    if (s.changed_bits[k] || !same_cmds)
+      fprintf(stderr, "verify: chunk %u [%u..%u) start %u: %u bits differ, out-state %s (ncmd %u/%u out_pos %u/%u)\n", k, s.bin[k].pos, s.bin[k].end,
+              s.bin[k].start_pos, s.changed_bits[k], same ? "same" : "DIFFERENT", a.ncmd, b.ncmd, a.out_pos, b.out_pos);
+  }
+  s.epoch = epoch0;
+  std::copy(old.begin(), old.end(), m.bout.begin()); std::copy(used0.begin(), used0.end(), m.bin_used.begin());
+  std::copy(old_cmds.begin(), old_cmds.end(), m.cmd_blocks.begin());
+  std::copy(latest0.begin(), latest0.end(), m.bits_latest.begin()); std::copy(srch0.begin(), srch0.end(), m.srch_latest.begin());
+  std::copy(counters0.begin(), counters0.end(), m.counters.begin()); std::copy(key_flips0.begin(), key_flips0.end(), m.key_flips.begin());
+  std::copy(saw0.begin(), saw0.end(), m.saw.begin()); std::copy(changed_bits0.begin(), changed_bits0.end(), m.changed_bits.begin());
+  std::copy(bitdep0.begin(), bitdep0.end(), m.bitdep_epoch.begin()); std::copy(changed_epoch0.begin(), changed_epoch0.end(), m.changed_epoch.begin());
+  std::copy(blks0.begin(), blks0.end(), m.blks.begin());
+  return ndiff;
 }
 
 // Runs the LZ77 stage; returns the commands of every metablock back to back.
@@ -276,7 +395,7 @@ extern "C" long sim_lz77(int q, int lgwin, const u8* in, u32 n, BrCmd* cmds_out,
                          u32* mb_info /* [5*i]: start,end,ncmd,compress,cmd_off */, u32 mb_cap, u32* stats) {
   SimStream* m = sim_setup(q, lgwin, in, n);
   if (!m) return -1;
-  sim_lz77_fixpoint(*m);
+  if (const int e = sim_lz77_fixpoint(*m)) { delete m; return e; }
   u32 nm = m->s.counters[1], total = m->s.counters[2];
   if (total > cmds_cap || nm > mb_cap) { delete m; return -2; }
   memcpy(cmds_out, m->cmds_all.data(), (size_t)total * sizeof(BrCmd));
@@ -378,16 +497,21 @@ static void sim_entropy2(SimStream& m, SimEnt& E) {
 }
 
 // Full pipeline; returns compressed size or negative error.  cuts: see br_pipeline.h BrCuts.
-static long sim_compress_impl(int q, int lgwin, const u8* in, u32 n, u8* out, size_t out_cap, u32* stats, const SimCuts* cuts) {
+// stats: nstats words (SIM_ST_*).
+static long sim_compress_impl(int q, int lgwin, const u8* in, u32 n, u8* out, size_t out_cap, u32* stats, const SimCuts* cuts,
+                              const SimSched* sched = nullptr, u32 nstats = SIM_ST_MODEL_COST + 1) {
   if (n == 0) { if (out_cap < 1) return -3; out[0] = 6; return 1; }
-  SimStream* m = sim_setup(q, lgwin, in, n, cuts);
+#ifdef BR_SIM_DEBUG
+  memset(br_sim_cnt, 0, sizeof(br_sim_cnt)); memset(br_sim_bnd, 0, sizeof(br_sim_bnd));
+#endif
+  SimStream* m = sim_setup(q, lgwin, in, n, cuts, sched);
   if (!m) return -1;
   BrStream& s = m->s;
   std::vector<u8> res;
   int rounds = 0;
   for (;;) {
     ++rounds;
-    sim_lz77_fixpoint(*m);
+    if (const int e = sim_lz77_fixpoint(*m)) { delete m; return e; }
     u32 nm = s.counters[1];
     SimEnt E;
     sim_entropy2(*m, E);
@@ -432,7 +556,12 @@ static long sim_compress_impl(int q, int lgwin, const u8* in, u32 n, u8* out, si
     }
     if (rounds > 64 + (int)s.P.multi) { delete m; return -4; }
   }
-  stats[0] = (u32)m->iterations; stats[1] = (u32)m->block_runs; stats[2] = s.P.nblocks; stats[3] = (u32)rounds; stats[4] = (u32)m->model_cost;
+  m->st[SIM_ST_LAUNCHES] = (u32)m->iterations; m->st[SIM_ST_WALKS] = (u32)m->block_runs; m->st[SIM_ST_CHUNKS] = s.P.nblocks;
+  m->st[SIM_ST_ROUNDS] = (u32)rounds; m->st[SIM_ST_MODEL_COST] = (u32)m->model_cost; m->st[SIM_ST_RAN_CAP] = m->ran_cap;
+#ifdef BR_SIM_DEBUG
+  m->st[SIM_ST_PREDICT_OK] = (u32)br_sim_bnd[0]; m->st[SIM_ST_PREDICT_NO] = (u32)br_sim_bnd[1];
+#endif
+  memcpy(stats, m->st, std::min<u32>(nstats, SIM_ST_WORDS) * sizeof(u32));
   delete m;
   if (res.size() > out_cap) return -3;
   memcpy(out, res.data(), res.size());
@@ -500,13 +629,35 @@ extern "C" long sim_q1_compress(int lgwin, const u8* in, u32 n, const size_t* ca
 #ifdef BR_SIM_ENTROPY
 // A batch of independent streams laid end to end (cuts of kind 3, br_pipeline.h): bounds[k] = end of stream k (bounds[ns-1] = n).
 // stream_end[k] receives the byte offset where stream k ends in `out`.
-extern "C" long sim_compress_multi(int q, int lgwin, const u8* in, u32 n, const u32* bounds, u32 nstreams, u64* stream_end,
-                                   u8* out, size_t out_cap, u32* stats) {
+static long sim_compress_multi_impl(int q, int lgwin, const u8* in, u32 n, const u32* bounds, u32 nstreams, u64* stream_end,
+                                    u8* out, size_t out_cap, u32* stats, const SimSched* sched, u32 nstats) {
   std::vector<u32> kind(nstreams, 3);
   u32 hint = 0;
   for (u32 k = 0; k < nstreams; ++k) { const u32 sz = bounds[k] - (k ? bounds[k - 1] : 0); if (sz > hint) hint = sz; }
   SimCuts c; memset(&c, 0, sizeof(c));
   c.pos = bounds; c.kind = kind.data(); c.n = nstreams - 1; c.is_final = 1; c.with_header = 1; c.size_hint = hint; c.stream_end = stream_end;
-  return sim_compress_impl(q, lgwin, in, n, out, out_cap, stats, &c);
+  return sim_compress_impl(q, lgwin, in, n, out, out_cap, stats, &c, sched, nstats);
+}
+extern "C" long sim_compress_multi(int q, int lgwin, const u8* in, u32 n, const u32* bounds, u32 nstreams, u64* stream_end,
+                                   u8* out, size_t out_cap, u32* stats) {
+  return sim_compress_multi_impl(q, lgwin, in, n, bounds, nstreams, stream_end, out, out_cap, stats, nullptr, SIM_ST_MODEL_COST + 1);
+}
+
+// The fixpoint under an explicit schedule (SimSched; its fields replace the BR_SIM_* switches).  One stream, optionally cut
+// (cut_pos / cut_kind / ncuts / size_hint as sim_compress_cuts, the stream finished, with its header), or a batch of streams when
+// every cut is of kind 3 (stream_end as sim_compress_multi).  stats: SIM_ST_WORDS words.  Returns the compressed size, or
+// a negative error (SIM_ERR_CAPACITY: a launch appended more entries than an array of the product holds).
+extern "C" long sim_compress_sched(int q, int lgwin, const u8* in, u32 n, const u32* cut_pos, const u32* cut_kind, u32 ncuts,
+                                   u32 size_hint, const SimSched* sched, u64* stream_end, u8* out, size_t out_cap, u32* stats) {
+  bool batch = ncuts > 0;
+  for (u32 i = 0; i < ncuts; ++i) batch = batch && cut_kind[i] == 3;
+  if (batch) {
+    std::vector<u32> bounds(cut_pos, cut_pos + ncuts); bounds.push_back(n);
+    return sim_compress_multi_impl(q, lgwin, in, n, bounds.data(), ncuts + 1, stream_end, out, out_cap, stats, sched, SIM_ST_WORDS);
+  }
+  if (ncuts == 0) return sim_compress_impl(q, lgwin, in, n, out, out_cap, stats, nullptr, sched, SIM_ST_WORDS);
+  SimCuts c; memset(&c, 0, sizeof(c));
+  c.pos = cut_pos; c.kind = cut_kind; c.n = ncuts; c.is_final = 1; c.with_header = 1; c.size_hint = size_hint;
+  return sim_compress_impl(q, lgwin, in, n, out, out_cap, stats, &c, sched, SIM_ST_WORDS);
 }
 #endif
