@@ -30,6 +30,31 @@ BR_DEV u32 br_chunk_of(const BrStream& s, u32 p) {
   return s.blk[b].first_chunk + ((p - s.blk[b].start) >> s.P.chunk_bits);
 }
 
+// Initial speculation for input block bi: every hashable position of the block is stored (true for > 99.8 % of text
+// positions, SURVEY.md appendix E).  Lane `lane` of `stride` ORs its words of the block into a zeroed bits_latest (words
+// shared by two blocks are ORed by both).
+BR_DEV void br_init_bits(const BrStream& s, u32 bi, u32 lane, u32 stride) {
+  const BrBlk B = s.blk[bi];
+  const u32 htl = s.P.htl;
+  // positions of this block that the parse stores: those with a full hash load inside the block ...
+  u32 lo = B.start, hi = B.end - B.start >= htl ? B.end - htl + 1 : B.start;
+  // ... and the last three, stored by StitchToPreviousBlock of the next block (hash_longest_match64_inc.h:127)
+  u32 s_lo = 0, s_hi = 0;
+  if (bi + 1 < s.nblk) {
+    const BrBlk N = s.blk[bi + 1];
+    if (N.end - N.start >= htl - 1 && N.start >= 3) { s_lo = N.start - 3 > B.start ? N.start - 3 : B.start; s_hi = N.start; }
+  }
+  const u32 w0 = B.start >> 5, w1 = (B.end - 1) >> 5;
+  for (u32 wi = w0 + lane; wi <= w1; wi += stride) {
+    u32 v = 0;
+    for (u32 b = 0; b < 32; ++b) {
+      const u32 p = wi * 32 + b;
+      if ((p >= lo && p < hi) || (p >= s_lo && p < s_hi)) v |= 1u << b;
+    }
+    if (v) br_atomic_or(s.bits_latest + wi, v);
+  }
+}
+
 // Compare and commit the stored-bits a walker just produced for chunk k (warp task).  The
 // walker owns the positions [start_pos, out_pos).  StitchToPreviousBlock of the FOLLOWING input
 // block (hash_longest_match64_inc.h:127) stores the last three positions of a block after its

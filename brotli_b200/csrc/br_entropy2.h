@@ -513,3 +513,23 @@ BR_DEV void br_emit_lit(const BrStream& st, const BrEnt& e, u32 o) {
   br_put_bits_at(out, off, swn, sw);
   br_put_bits_at(out, off + swn, n, code);
 }
+
+#include <vector>
+// Host: where every metablock's scratch (bytes) and bit buffer (words) start -- only compressed metablocks take room --
+// and how many bytes the assembled stream may take.
+struct BrMbLayout {
+  std::vector<u64> scratch_off, out_off;
+  size_t scratch_bytes, out_words, out_cap;
+};
+static inline void br_mb_layout(const BrParams& P, const BrMetaBlock* mbs, u32 n_mbs, BrMbLayout& L) {
+  L.scratch_off.assign(n_mbs, 0); L.out_off.assign(n_mbs, 0);
+  L.scratch_bytes = L.out_words = 0;
+  for (u32 i = 0; i < n_mbs; ++i) {
+    L.scratch_off[i] = L.scratch_bytes; L.out_off[i] = L.out_words;
+    if (mbs[i].compress) {
+      L.scratch_bytes += ((size_t)br_mb_scratch_bytes(P, mbs[i].nlit, mbs[i].ncmd) + 255) & ~(size_t)255;
+      L.out_words += (2 * (size_t)(mbs[i].end - mbs[i].start) + 503) / 4 + 16;
+    }
+  }
+  L.out_cap = (size_t)P.n + ((size_t)P.n >> 3) + 4096 + 8ull * n_mbs;
+}

@@ -200,9 +200,9 @@ __global__ void k_seg(const KT* __restrict__ sorted_keys, u32 n, u32 nbuckets, u
 }
 
 // Buffers of the position index (n elements each unless noted).  Qualities 5..9 use K1, V1, K2; qualities 2..4 the four
-// 32-bit arrays qk_*.
+// 32-bit arrays qk_*.  tagS is filled by k_tags.
 struct BrIndexBufs {
-  u16 *K1, *K2;                              // K2: the sorted bucket keys (BrStream::skeys)
+  u16 *K1, *K2, *tagS;                       // K2: the sorted bucket keys (BrStream::skeys)
   u32 *V1, *S, *rank, *seg;                  // seg: nbuckets + 2 words
   u32 *hist, *scan_tmp;                      // 256 * ntiles words and scan_tmp_words of that
   u32 *qk_keys, *qk_K1, *qk_V1, *qk_V2;
@@ -265,30 +265,8 @@ static void scan_exclusive(u32* a, u32 n, u32* tmp, cudaStream_t st) {
 }
 
 // ---------------------------------------------------------------------------- stored bits
-// Initial speculation: every hashable position of a block is stored (true for > 99.8 % of
-// text positions, SURVEY.md appendix E).  One CTA per input block (blocks cut by a FLUSH are irregular); words shared
-// by two blocks are ORed into a zeroed bitmap.
-__global__ void k_init_bits(BrStream s) {
-  const BrBlk B = s.blk[blockIdx.x];
-  const u32 htl = s.P.htl;
-  // positions of this block that the parse stores: those with a full hash load inside the block ...
-  u32 lo = B.start, hi = B.end - B.start >= htl ? B.end - htl + 1 : B.start;
-  // ... and the last three, stored by StitchToPreviousBlock of the next block (hash_longest_match64_inc.h:127)
-  u32 s_lo = 0, s_hi = 0;
-  if (blockIdx.x + 1 < s.nblk) {
-    const BrBlk N = s.blk[blockIdx.x + 1];
-    if (N.end - N.start >= htl - 1 && N.start >= 3) { s_lo = N.start - 3 > B.start ? N.start - 3 : B.start; s_hi = N.start; }
-  }
-  const u32 w0 = B.start >> 5, w1 = (B.end - 1) >> 5;
-  for (u32 wi = w0 + threadIdx.x; wi <= w1; wi += blockDim.x) {
-    u32 v = 0;
-    for (u32 b = 0; b < 32; ++b) {
-      const u32 p = wi * 32 + b;
-      if ((p >= lo && p < hi) || (p >= s_lo && p < s_hi)) v |= 1u << b;
-    }
-    if (v) atomicOr(s.bits_latest + wi, v);
-  }
-}
+// Initial speculation (br_chain.h br_init_bits): one CTA per input block (blocks cut by a FLUSH are irregular).
+__global__ void k_init_bits(BrStream s) { br_init_bits(s, blockIdx.x, threadIdx.x, blockDim.x); }
 // bits_latest permuted into S order + per-1024 popcounts: the first snapshot of a job (br_snapshot_update keeps it)
 __global__ void __launch_bounds__(1024) k_build_storedS(BrStream s, u32* __restrict__ storedS, u32* __restrict__ blockcnt) {
   __shared__ u32 wsum[32];
@@ -311,18 +289,9 @@ __global__ void k_snapshot_update(BrStream s, u32* __restrict__ storedS, u32* __
 }
 
 // ---------------------------------------------------------------------------- warp-task kernels
-// G = bucket-ring rows fetched together (br_lz77.h): 1 for the 16/32-entry rings of quality 5-6 (throughput bound,
-// 8 CTAs per SM), 4 for the 64-256-entry rings of quality 7-9 (more registers, fewer resident warps).
+// k_walk<G, M>: G and M as br_walk_dispatch (br_params.h) picks them
 #ifndef BR_WALK1_MINB
 #define BR_WALK1_MINB 8
-#endif
-#ifndef BR_WALK_G_DEEP
-#define BR_WALK_G_DEEP 4    /* rows fetched together for the 256-entry rings of quality 9: 8 (the whole ring, 125 registers,
-                               16 warps per SM) walks one chunk faster, 4 (96 registers, 20 warps per SM) won on the whole
-                               job of config C4 when the two were timed against each other */
-#endif
-#ifndef BR_WALK_G_SMALL
-#define BR_WALK_G_SMALL 1   /* rows fetched together for the 16/32-entry rings */
 #endif
 template <int G, bool M>
 __global__ void __launch_bounds__(128, G <= 2 ? BR_WALK1_MINB : G == 4 ? 5 : 4) k_walk(BrStream s) {
@@ -537,22 +506,34 @@ static BrDeviceTables* get_tables() {
 
 // Grow-only device arena owned by a job; all per-stream arrays are carved out of it.
 struct BrArena {
-  u8* base = nullptr; size_t cap = 0, used = 0;
+  u8* base = nullptr; size_t cap = 0;
   bool reserve(size_t bytes) {
-    if (bytes <= cap) { used = 0; return true; }
+    if (bytes <= cap) return true;
     if (base) cudaFree(base);
     base = nullptr; cap = 0;
     if (cudaMalloc(&base, bytes) != cudaSuccess) { cudaGetLastError(); return false; }
-    cap = bytes; used = 0; return true;
-  }
-  template <class T> T* take(size_t count) {
-    size_t off = (used + 255) & ~(size_t)255;
-    used = off + count * sizeof(T);
-    if (used > cap) return nullptr;
-    return (T*)(base + off);
+    cap = bytes; return true;
   }
   void release() { if (base) cudaFree(base); base = nullptr; cap = 0; }
 };
+// Lays arrays out one behind the other, 256-byte aligned, from base; with base == nullptr it only counts the bytes.
+struct BrCarve {
+  u8* base; size_t used;
+  template <class T> T* take(size_t count) {
+    const size_t off = (used + 255) & ~(size_t)255;
+    used = off + count * sizeof(T);
+    return base ? (T*)(base + off) : nullptr;
+  }
+};
+// Every arena is laid out by one function, carve(BrCarve&), run twice: to measure, then to assign from the arena.
+template <class F> static bool br_carve(BrArena& A, F&& carve) {
+  BrCarve m{nullptr, 0};
+  carve(m);
+  if (!A.reserve(m.used)) return false;
+  BrCarve c{A.base, 0};
+  carve(c);
+  return true;
+}
 
 struct BrJob {
   cudaStream_t st = nullptr;
@@ -583,6 +564,20 @@ extern "C" void* br_job_stream(BrJob* j) { return (void*)j->st; }
 
 static size_t scan_tmp_words(size_t n) { return n / SCAN_CHUNK + n / SCAN_CHUNK / SCAN_CHUNK + 64; }
 
+// The position index's arrays and tagS, in arena order; at qualities 2..4 carve_index_quick adds the 32-bit sort arrays.
+static void carve_index(BrCarve& A, const BrParams& P, BrIndexBufs& b) {
+  const size_t n = P.n, ntiles = (n + RADIX_TILE - 1) / RADIX_TILE;
+  b.K1 = A.take<u16>(n + 2); b.V1 = A.take<u32>(n);
+  b.K2 = A.take<u16>(n + 2); b.S = A.take<u32>(n); b.rank = A.take<u32>(n); b.tagS = A.take<u16>(n + 2);
+  b.hist = A.take<u32>(256 * ntiles); b.scan_tmp = A.take<u32>(scan_tmp_words(256 * ntiles));
+  b.seg = A.take<u32>(P.nbuckets + 4);
+}
+static void carve_index_quick(BrCarve& A, const BrParams& P, BrIndexBufs& b) {
+  if (!P.quick) return;
+  const size_t n = P.n;
+  b.qk_keys = A.take<u32>(n + 4); b.qk_K1 = A.take<u32>(n + 4); b.qk_V1 = A.take<u32>(n + 4); b.qk_V2 = A.take<u32>(n + 4);
+}
+
 // Compress one stream whose input already sits in device memory (d_in, n bytes).  The
 // compressed bytes are left in device memory (*d_out, *out_size; valid until the next call on
 // this job).  Returns 1 on success, 0 on failure (unsupported parameters, CUDA error).
@@ -591,12 +586,12 @@ static size_t scan_tmp_words(size_t n) { return n / SCAN_CHUNK + n / SCAN_CHUNK 
 static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const u8* d_in, u32 n, const u8** d_out, size_t* out_size,
                         const BrCuts* cuts, const BrSchedKnobs* knobs) {
   BrDeviceTables* T = get_tables();
-  if (!T || n == 0) return 0;
+  if (!T) return 0;
+  BrStreamPlan plan;
+  if (!br_plan_stream(quality, lgwin, size_hint, n, cuts, knobs, &plan)) return 0;
   BrStream s; memset(&s, 0, sizeof(s));
-  if (!br_derive_params(quality, lgwin, size_hint, n, &s.P, cuts ? cuts->lgblock : 0)) return 0;
+  s.P = plan.P;
   BrParams& P = s.P;
-  P.disable_ctx = cuts && cuts->disable_ctx ? 1u : 0u;
-  P.stream_offset = cuts ? (cuts->stream_offset < P.max_backward ? cuts->stream_offset : P.max_backward) : 0u;   // encode.c:680
 #ifdef BR_DEBUG_KNOBS   // experiment switches: never in the release build (an environment variable must not change the bytes)
   if (getenv("BR_HEAVY_MIN")) P.heavy_min = (u32)strtoul(getenv("BR_HEAVY_MIN"), 0, 10);
   if (getenv("BR_STEP_CAP")) P.step_cap = (u32)strtoul(getenv("BR_STEP_CAP"), 0, 10);
@@ -606,162 +601,90 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
 #else
   const bool trace = false;
 #endif
-  if (knobs) {
-    if (knobs->sweep_epoch != BR_KNOB_KEEP) P.sweep_epoch = knobs->sweep_epoch;
-    if (knobs->force_epoch != BR_KNOB_KEEP) P.force_epoch = knobs->force_epoch;
-    if (knobs->step_cap != BR_KNOB_KEEP) P.step_cap = knobs->step_cap;
-    if (knobs->heavy_min != BR_KNOB_KEEP) P.heavy_min = knobs->heavy_min;
-    if (knobs->pilot != BR_KNOB_KEEP) P.pilot = knobs->pilot;
-    if (knobs->sweep_blocks != BR_KNOB_KEEP) {
-      if (knobs->sweep_blocks == 0 || (knobs->sweep_blocks & (knobs->sweep_blocks - 1))) return 0;   // (a power of two)
-      P.sweep_blocks = knobs->sweep_blocks;
-    }
-  }
-  // chunk / block tables: the reference's input blocks (1 << lgblock bytes, shorter where a FLUSH cut the input)
-  std::vector<BrBlk> hblk;
-  const u32 ncuts = cuts ? cuts->n : 0;
-  u32 nstreams = 1;
-  for (u32 i = 0; i < ncuts; ++i) if (cuts->kind[i] == 3) ++nstreams;
-  if (nstreams > 1) {
-    // a batch of independent streams (each below BR_SMALL_STREAM, size_hint = the largest): no FLUSH cuts, all finished
-    if (nstreams != ncuts + 1 || !cuts->is_final || !cuts->with_header || cuts->finish_empty || cuts->stream_offset ||
-        cuts->pos[ncuts - 1] >= n || size_hint >= BR_SMALL_STREAM) return 0;
-    P.multi = nstreams; P.pilot = 0;
-    P.chunk_bits = br_batch_chunk_bits(n);
-  }
-  if (P.quick && P.stream_offset) return 0;   // (STREAM_OFFSET: quality 5..9)
+  const u32 nb = P.nblocks, nblk = (u32)plan.blk.size(), ncuts = cuts ? cuts->n : 0, nstreams = plan.nstreams;
   const u32 ch = 1u << P.chunk_bits;
-  const bool is_final = cuts ? cuts->is_final != 0 : true;
-  const int with_header = cuts ? cuts->with_header : 1;
-  P.finish_empty = cuts && cuts->finish_empty ? 1u : 0u;
-  if (!is_final && (ncuts == 0 || cuts->pos[ncuts - 1] != n)) return 0;   // an unfinished stream ends at a cut
-  if (P.finish_empty && (!is_final || (ncuts && cuts->pos[ncuts - 1] == n))) return 0;
-  u32 nb = 0;
-  br_build_blocks(P, n, cuts ? cuts->pos : nullptr, ncuts, is_final && !P.finish_empty, nullptr, hblk, &nb, cuts ? cuts->kind : nullptr);   // chunks: k_build_chunks
-  std::vector<u32> h_slot(((size_t)n >> P.lgblock) + 2, 0);
-  { u32 b = 0; for (size_t i = 0; i < h_slot.size(); ++i) { const u64 p = (u64)i << P.lgblock; while (b + 1 < hblk.size() && hblk[b].end <= p) ++b; h_slot[i] = b; } }
-  const u32 nblk = (u32)hblk.size();
-  P.nblocks = nb;
   cudaStream_t st = job->st;
   memset(&job->stats, 0, sizeof(job->stats));
+  job->stats.ran_cap = plan.ran_cap;
   cudaEvent_t* ev = job->ev;
   cudaEventRecord(ev[0], st);
 
-  const u32 ntiles = (n + RADIX_TILE - 1) / RADIX_TILE;
   const size_t nwords = (size_t)(n + 31) / 32 + 2;
-  const u32 cmd_stride = ch / 2 + 2;
-  size_t need = 0;
-  auto add = [&](size_t bytes) { need += (bytes + 255) & ~(size_t)255; };
-  add((size_t)n + 64); add(2ull * n + 4); add(4ull * n); add(2ull * n + 4); add(4ull * n); add(4ull * n); add(2ull * n + 4);
-  add(256ull * ntiles * 4); add(scan_tmp_words(256ull * ntiles) * 4);
-  add((P.nbuckets + 4) * 4ull); add(nwords * 4); add(2 * nwords * 4); add(nwords * 4); add(nwords * 4); add(nwords * 4); add(nwords * 4); add(nwords * 4); add((nwords + 64) * 4); add(((size_t)n / 1024 + 8) * 4); add(((size_t)n / 1024 + 8) * 4);
-  add(scan_tmp_words((size_t)n / 1024 + 8) * 4);
-  add(nb * sizeof(BrBlockIn) * 2); add(nb * sizeof(BrBlockOut)); add((size_t)nb * cmd_stride * sizeof(BrCmd));
-  for (int i = 0; i < 14; ++i) add(nb * 4ull + 64);
-  add(nblk * sizeof(BrBlk)); add(nblk * sizeof(BrBlkIn)); add((P.nbuckets + 8) * 4ull);
-  add(h_slot.size() * 4); add((ncuts + 2) * 4ull); add((ncuts + 2) * 8ull); add((nstreams + 2) * 8ull);
-  add((nstreams + 2) * 4ull * 3); add(nblk * sizeof(BrMetaBlock)); add(1024ull * nstreams);
-  // Launch bound: in forced mode every launch finalises at least one input block (at most two launches per block with
-  // the conservative block-level re-marks), and a late uncompressed fallback restarts the count at most once per metablock.
-  P.max_epochs = 4 * nb + 4096;
-  add(((size_t)P.max_epochs + 2) * 4 + 64); add((nb + 1) * sizeof(BrMetaBlock)); add(4096);
-  if (P.quick) { for (int i = 0; i < 4; ++i) add(4ull * n + 16); add((((size_t)n << P.qk_sweep_bits) + 16) * 4); add((((size_t)n << P.qk_sweep_bits) + 16) * 4); }   // 32-bit sort keys, slot entry points, slot reads
-  need += 1 << 20;
-  if (!job->arena.reserve(need)) return 0;
-  BrArena& A = job->arena;
-  u8* data = A.take<u8>((size_t)n + 64);
-  u16* K1 = A.take<u16>((size_t)n + 2); u32* V1 = A.take<u32>(n);
-  u16* K2 = A.take<u16>((size_t)n + 2); u32* S = A.take<u32>(n); u32* rank = A.take<u32>(n); u16* tagS = A.take<u16>((size_t)n + 2);
-  u32* hist = A.take<u32>(256ull * ntiles); u32* scan_tmp = A.take<u32>(scan_tmp_words(256ull * ntiles));
-  u32* seg = A.take<u32>(P.nbuckets + 4);
-  u32* bits_latest = A.take<u32>(nwords); u32* bits_cur = A.take<u32>(2 * (size_t)nwords);
-  u32* srch_latest = A.take<u32>(nwords); u32* srch_cur = A.take<u32>(nwords); u32* bits_prev = A.take<u32>(nwords);
-  u32* cover_cur = A.take<u32>(nwords);
-  u32* storedS = A.take<u32>(nwords + 64); u32* prefS = A.take<u32>((size_t)n / 1024 + 8); u32* cntS = A.take<u32>((size_t)n / 1024 + 8);
-  u32* scan_tmp2 = A.take<u32>(scan_tmp_words((size_t)n / 1024 + 8));
-  BrBlockIn* bin = A.take<BrBlockIn>(nb); BrBlockIn* bin_used = A.take<BrBlockIn>(nb);
-  BrBlockOut* bout = A.take<BrBlockOut>(nb);
-  BrCmd* cmd_blocks = A.take<BrCmd>((size_t)nb * cmd_stride);
-  u32* dirty = A.take<u32>(nb + 16); u32* changed_bits = A.take<u32>(nb + 16);
-  int* changed_epoch = A.take<int>(nb + 16); u32* ext_total = A.take<u32>(nb + 16);
-  u32* cmd_off = A.take<u32>(nb + 16); u32* force_unc = A.take<u32>(nb + 16);
-  u32* dirty_list = A.take<u32>(nb + 16); u32* block_mb = A.take<u32>(nb + 16);
-  // ran_list: every chunk is walked at most once per launch -- by its own scheduled walker or by the one sweep that chases
-  // into it, and in a forced launch the walkers scheduled behind the forced one in its input block stand down
-  // (br_walk_block) -- so a launch appends at most nb entries
-  u32* ran_list = A.take<u32>(nb + 16); u32* lil_in = A.take<u32>(nb + 16);
-  job->stats.ran_cap = nb + 16;
-  int* bitdep_epoch = A.take<int>(nb + 16);
-  BrBlk* d_blk = A.take<BrBlk>(nblk); BrBlkIn* d_blkin = A.take<BrBlkIn>(nblk);
-  u32* key_flips = A.take<u32>(P.nbuckets + 8);
-  u32* slot_blk = A.take<u32>(h_slot.size()); u32* d_cut_kind = A.take<u32>(ncuts + 2); u64* d_cut_end = A.take<u64>(ncuts + 2);
-  u64* d_stream_end = A.take<u64>(nstreams + 2);
-  u32* epoch_cum = A.take<u32>((size_t)P.max_epochs + 2);
-  BrMetaBlock* mbs = A.take<BrMetaBlock>(nb + 1);
-  u32* d_stream_blk = A.take<u32>(nstreams + 2); u32* stream_nmb = A.take<u32>(nstreams + 2); u32* stream_ncmd = A.take<u32>(nstreams + 2);
-  BrMetaBlock* mbs_stage = A.take<BrMetaBlock>(nblk);
-  u32* counters = A.take<u32>(64); u32* hist_scratch = A.take<u32>(256ull * nstreams);
-  if (!hist_scratch) return 0;
-  u32 *qk_keys = nullptr, *qk_K1 = nullptr, *qk_V1 = nullptr, *qk_V2 = nullptr, *saw = nullptr, *qpred = nullptr;
-  if (P.quick) {
-    qk_keys = A.take<u32>((size_t)n + 4); qk_K1 = A.take<u32>((size_t)n + 4); qk_V1 = A.take<u32>((size_t)n + 4); qk_V2 = A.take<u32>((size_t)n + 4);
-    saw = A.take<u32>(((size_t)n << P.qk_sweep_bits) + 16);
-    qpred = A.take<u32>(((size_t)n << P.qk_sweep_bits) + 16);
-    if (!qpred) return 0;
-  }
-  s.saw = saw; s.qpred = qpred;
+  s.bits_words = (u32)nwords; s.cmd_stride = plan.cmd_stride; s.nblk = nblk;
+  BrIndexBufs ix;
+  u32 *cntS, *scan_tmp2, *cut_kind;
+  u64 *cut_end, *stream_end;
+  auto carve = [&](BrCarve& A) {
+    s.data = A.take<u8>((size_t)n + 64);
+    carve_index(A, P, ix);
+    s.bits_latest = A.take<u32>(nwords); s.bits_cur = A.take<u32>(2 * nwords);
+    s.srch_latest = A.take<u32>(nwords); s.srch_cur = A.take<u32>(nwords); s.bits_prev = A.take<u32>(nwords);
+    s.cover_cur = A.take<u32>(nwords);
+    s.storedS = A.take<u32>(nwords + 64); s.prefS = A.take<u32>((size_t)n / 1024 + 8); cntS = A.take<u32>((size_t)n / 1024 + 8);
+    scan_tmp2 = A.take<u32>(scan_tmp_words((size_t)n / 1024 + 8));
+    s.bin = A.take<BrBlockIn>(nb); s.bin_used = A.take<BrBlockIn>(nb);
+    s.bout = A.take<BrBlockOut>(nb);
+    s.cmd_blocks = A.take<BrCmd>((size_t)nb * plan.cmd_stride);
+    s.dirty = A.take<u32>(nb + 16); s.changed_bits = A.take<u32>(nb + 16);
+    s.changed_epoch = A.take<int>(nb + 16); s.ext_total = A.take<u32>(nb + 16);
+    s.cmd_off = A.take<u32>(nb + 16); s.force_unc = A.take<u32>(nb + 16);
+    s.dirty_list = A.take<u32>(nb + 16); s.block_mb = A.take<u32>(nb + 16);
+    s.ran_list = A.take<u32>(plan.ran_cap); s.lil_in = A.take<u32>(nb + 16);
+    s.bitdep_epoch = A.take<int>(nb + 16);
+    s.blk = A.take<BrBlk>(nblk); s.blkin = A.take<BrBlkIn>(nblk);
+    s.key_flips = A.take<u32>(P.nbuckets + 8);
+    s.slot_blk = A.take<u32>(plan.slot_blk.size()); cut_kind = A.take<u32>(ncuts + 2); cut_end = A.take<u64>(ncuts + 2);
+    stream_end = A.take<u64>(nstreams + 2);
+    s.epoch_cum = A.take<u32>((size_t)P.max_epochs + 2);
+    s.mbs = A.take<BrMetaBlock>(nb + 1);
+    s.stream_blk = A.take<u32>(nstreams + 2); s.stream_nmb = A.take<u32>(nstreams + 2); s.stream_ncmd = A.take<u32>(nstreams + 2);
+    s.mbs_stage = A.take<BrMetaBlock>(nblk);
+    s.counters = A.take<u32>(64); s.hist_scratch = A.take<u32>(256ull * nstreams);
+    if (P.quick) {   // 32-bit sort keys, slot reads, slot entry points
+      carve_index_quick(A, P, ix);
+      s.saw = A.take<u32>(((size_t)n << P.qk_sweep_bits) + 16);
+      s.qpred = A.take<u32>(((size_t)n << P.qk_sweep_bits) + 16);
+    }
+  };
+  if (!br_carve(job->arena, carve)) return 0;
+  s.S = ix.S; s.rank = ix.rank; s.seg = ix.seg; s.skeys = ix.K2; s.tagS = ix.tagS;
+  br_bind_tables(s, T->blob, T->log2tab, T->log2tab_n);
 
-  CK(cudaMemcpyAsync(data, d_in, n, cudaMemcpyDeviceToDevice, st));
-  CK(cudaMemsetAsync(data + n, 0, 64, st));
-  s.data = data; s.S = S; s.rank = rank; s.seg = seg; s.bits_latest = bits_latest; s.bits_cur = bits_cur; s.bits_words = (u32)nwords;
-  s.storedS = storedS; s.prefS = prefS; s.bin = bin; s.bin_used = bin_used; s.bout = bout;
-  s.cmd_blocks = cmd_blocks; s.cmd_stride = cmd_stride; s.dirty = dirty; s.changed_bits = changed_bits;
-  s.changed_epoch = changed_epoch; s.epoch_cum = epoch_cum;
-  s.ext_total = ext_total; s.cmd_off = cmd_off; s.mbs = mbs; s.force_unc = force_unc;
-  s.counters = counters; s.hist_scratch = hist_scratch;
-  s.srch_latest = srch_latest; s.srch_cur = srch_cur; s.bits_prev = bits_prev; s.cover_cur = cover_cur; s.bitdep_epoch = bitdep_epoch; s.skeys = K2;
-  s.dirty_list = dirty_list; s.block_mb = block_mb; s.ran_list = ran_list; s.lil_in = lil_in; s.blk = d_blk; s.nblk = nblk; s.blkin = d_blkin; s.key_flips = key_flips;
-  { const u8* p = T->blob + 8;
-    s.dict_size_bits = p; p += 32; s.dict_offsets = (const u32*)p; p += 128; s.dict = p; p += 122784;
-    s.dict_hash_words = (const u16*)p; p += 65536; s.dict_hash_lengths = p; p += 32768; s.ctx_lut = p; }
-  s.log2tab = T->log2tab; s.log2tab_n = T->log2tab_n;
-
-  CK(cudaMemcpyAsync(d_blk, hblk.data(), nblk * sizeof(BrBlk), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(slot_blk, h_slot.data(), h_slot.size() * 4, cudaMemcpyHostToDevice, st));
-  std::vector<u32> h_stream_blk(nstreams + 1, nblk);
-  for (u32 bi = nblk; bi-- > 0;) h_stream_blk[hblk[bi].stream] = bi;
-  CK(cudaMemcpyAsync(d_stream_blk, h_stream_blk.data(), (nstreams + 1) * 4ull, cudaMemcpyHostToDevice, st));
-  s.stream_blk = d_stream_blk; s.stream_nmb = stream_nmb; s.stream_ncmd = stream_ncmd; s.mbs_stage = mbs_stage;
-  if (ncuts) CK(cudaMemcpyAsync(d_cut_kind, cuts->kind, ncuts * 4, cudaMemcpyHostToDevice, st));
-  s.slot_blk = slot_blk;
-  CK(cudaMemsetAsync(bin, 0, nb * sizeof(BrBlockIn), st));
-  k_build_chunks<<<nblk, 64, 0, st>>>(d_blk, bin, 1u << P.chunk_bits);
-  CK(cudaStreamSynchronize(st));   // (hblk / h_slot are host vectors: their copies must be done before they go out of scope ... and before the arrays below are reused)
-  CK(cudaMemsetAsync(bout, 0, nb * sizeof(BrBlockOut), st));
-  CK(cudaMemsetAsync(bin_used, 0, nb * sizeof(BrBlockIn), st));
-  CK(cudaMemsetAsync(changed_bits, 0, (nb + 16) * 4, st));
-  CK(cudaMemsetAsync(changed_epoch, 0xFF, (nb + 16) * 4, st));
-  CK(cudaMemsetAsync(bitdep_epoch, 0xFF, (nb + 16) * 4, st));
-  CK(cudaMemsetAsync(srch_latest, 0, nwords * 4, st));
-  CK(cudaMemsetAsync(key_flips, 0, (P.nbuckets + 8) * 4, st));
-  CK(cudaMemsetAsync(force_unc, 0, (nb + 16) * 4, st));
-  CK(cudaMemsetAsync(epoch_cum, 0, 64, st));
-  CK(cudaMemsetAsync(counters, 0, 256, st));
-  CK(cudaMemsetAsync(bits_cur, 0, 2 * (size_t)nwords * 4, st));
+  CK(cudaMemcpyAsync((u8*)s.data, d_in, n, cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemsetAsync((u8*)s.data + n, 0, 64, st));
+  CK(cudaMemcpyAsync(s.blk, plan.blk.data(), nblk * sizeof(BrBlk), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync((u32*)s.slot_blk, plan.slot_blk.data(), plan.slot_blk.size() * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync((u32*)s.stream_blk, plan.stream_blk.data(), (nstreams + 1) * 4ull, cudaMemcpyHostToDevice, st));
+  if (ncuts) CK(cudaMemcpyAsync(cut_kind, cuts->kind, ncuts * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(s.bin, 0, nb * sizeof(BrBlockIn), st));
+  k_build_chunks<<<nblk, 64, 0, st>>>(s.blk, s.bin, ch);
+  CK(cudaStreamSynchronize(st));   // (the copies from the plan's host tables must be done before the arrays below are reused)
+  CK(cudaMemsetAsync(s.bout, 0, nb * sizeof(BrBlockOut), st));
+  CK(cudaMemsetAsync(s.bin_used, 0, nb * sizeof(BrBlockIn), st));
+  CK(cudaMemsetAsync(s.changed_bits, 0, (nb + 16) * 4, st));
+  CK(cudaMemsetAsync(s.changed_epoch, 0xFF, (nb + 16) * 4, st));
+  CK(cudaMemsetAsync(s.bitdep_epoch, 0xFF, (nb + 16) * 4, st));
+  CK(cudaMemsetAsync(s.srch_latest, 0, nwords * 4, st));
+  CK(cudaMemsetAsync(s.key_flips, 0, (P.nbuckets + 8) * 4, st));
+  CK(cudaMemsetAsync(s.force_unc, 0, (nb + 16) * 4, st));
+  CK(cudaMemsetAsync(s.epoch_cum, 0, 64, st));
+  CK(cudaMemsetAsync(s.counters, 0, 256, st));
+  CK(cudaMemsetAsync(s.bits_cur, 0, 2 * (size_t)nwords * 4, st));
 
   // ---- position index: S, rank, seg
-  br_build_index(P, data, d_blk, nblk, BrIndexBufs{K1, K2, V1, S, rank, seg, hist, scan_tmp, qk_keys, qk_K1, qk_V1, qk_V2}, st);
-  if (P.quick) k_slot_pred<<<nblk, 256, 0, st>>>(s, qpred);   // (s.S / s.rank / s.seg / s.blk / s.data are set; the kernel reads nothing else)
+  br_build_index(P, s.data, s.blk, nblk, ix, st);
+  if (P.quick) k_slot_pred<<<nblk, 256, 0, st>>>(s, (u32*)s.qpred);   // (the kernel reads s.S / s.rank / s.seg / s.blk / s.data only)
   // (the 16/32-entry rings of quality 5-6 gained nothing from tags when timed on C2, so only the deep rings of quality 7-9,
   // where most of the 256 ring entries are hash collisions whose bytes need not be fetched, use them)
-  if (P.block_bits >= 6) k_tags<<<(n + 255) / 256, 256, 0, st>>>(data, S, n, tagS);
-  s.tagS = tagS;
-  CK(cudaMemsetAsync(bits_latest, 0, nwords * 4, st));
+  if (P.block_bits >= 6) k_tags<<<(n + 255) / 256, 256, 0, st>>>(s.data, ix.S, n, ix.tagS);
+  CK(cudaMemsetAsync(s.bits_latest, 0, nwords * 4, st));
   k_init_bits<<<nblk, 256, 0, st>>>(s);
   cudaEventRecord(ev[1], st);
   // the S-ordered snapshot of the stored bits, for the bucket rings of quality 5..9: built once here, then carried along by
   // k_snapshot_update after every launch's commits
   const u32 nsnap = (n + 1023) / 1024;
+  u32* const storedS = (u32*)s.storedS;
+  u32* const prefS = (u32*)s.prefS;
   auto refresh_prefS = [&]() {
     cudaMemcpyAsync(prefS, cntS, nsnap * 4ull, cudaMemcpyDeviceToDevice, st);
     scan_exclusive(prefS, nsnap, scan_tmp2, st);
@@ -789,7 +712,7 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
       } else k_chain_b<<<1, 32, 0, st>>>(s);
       k_chain_c<<<(nblk + 31) / 32, 32, 0, st>>>(s);
       k_chain_d<<<(nb + 255) / 256, 256, 0, st>>>(s);
-      CK(cudaMemcpyAsync(hp, counters, 128, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(hp, s.counters, 128, cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
       u32 n_dirty = hp[0], n_sched = hp[5]; n_mbs = hp[1]; total_cmds = hp[2];
       job->stats.block_runs += hp[4];
@@ -804,26 +727,19 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
       ++s.epoch; ++job->stats.lz77_iterations;
       s.forced = s.epoch - round_epoch0 >= P.force_epoch ? 1u : 0u;
       job->stats.forced_launches += s.forced;
-      CK(cudaMemsetAsync(bits_cur, 0, 2 * (size_t)nwords * 4, st));
-      CK(cudaMemsetAsync(srch_cur, 0, nwords * 4, st));
-      CK(cudaMemsetAsync(counters + 4, 0, 4, st));
-      CK(cudaMemsetAsync(counters + 16, 0, 4, st));
+      CK(cudaMemsetAsync(s.bits_cur, 0, 2 * (size_t)nwords * 4, st));
+      CK(cudaMemsetAsync(s.srch_cur, 0, nwords * 4, st));
+      CK(cudaMemsetAsync(s.counters + 4, 0, 4, st));
+      CK(cudaMemsetAsync(s.counters + 16, 0, 4, st));
       cudaEventRecord(ev[6], st);
       const u32 wg = (n_sched + 3) / 4;
-      if (P.quick) {
-        if (P.multi) k_walk<0, true><<<wg, 128, 0, st>>>(s);
-        else k_walk<0, false><<<wg, 128, 0, st>>>(s);
-      } else if (P.multi) {
-        if (P.block_bits >= 6) k_walk<BR_WALK_G_DEEP, true><<<wg, 128, 0, st>>>(s);
-        else k_walk<BR_WALK_G_SMALL, true><<<wg, 128, 0, st>>>(s);
-      } else if (P.block_bits >= 6) k_walk<BR_WALK_G_DEEP, false><<<wg, 128, 0, st>>>(s);
-      else k_walk<BR_WALK_G_SMALL, false><<<wg, 128, 0, st>>>(s);
+      br_walk_dispatch(P, [&](auto g, auto m) { k_walk<decltype(g)::value, decltype(m)::value><<<wg, 128, 0, st>>>(s); });
       cudaEventRecord(ev[7], st);
       walk_pending = true; ++job->stats.walk_launches; job->stats.launches += 6;
       job->stats.walk_bytes += (u64)n_sched * ch;
-      CK(cudaMemcpyAsync(bits_prev, bits_latest, nwords * 4, cudaMemcpyDeviceToDevice, st));
+      CK(cudaMemcpyAsync((u32*)s.bits_prev, s.bits_latest, nwords * 4, cudaMemcpyDeviceToDevice, st));
       if (!P.quick) {   // (quality 2..4 check every run instead of marking: br_verify_run)
-        CK(cudaMemsetAsync(cover_cur, 0, nwords * 4, st));
+        CK(cudaMemsetAsync(s.cover_cur, 0, nwords * 4, st));
         k_cover<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s);
       }
       k_commit<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s);
@@ -837,7 +753,7 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
 #ifdef BR_DEBUG_KNOBS
     if (trace) {   // the slowest chunk walks of the final state, and a per-megabyte profile
       std::vector<BrBlockOut> hb2(nb);
-      cudaMemcpyAsync(hb2.data(), bout, nb * sizeof(BrBlockOut), cudaMemcpyDeviceToHost, st); cudaStreamSynchronize(st);
+      cudaMemcpyAsync(hb2.data(), s.bout, nb * sizeof(BrBlockOut), cudaMemcpyDeviceToHost, st); cudaStreamSynchronize(st);
       const u32 per = (1u << 20) >> P.chunk_bits;
       for (u32 a = 0; a < nb; a += per) {
         unsigned long long cyc = 0, se = 0, ro = 0; u32 mx = 0;
@@ -848,39 +764,31 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
 #endif
     // ---- entropy stage
     std::vector<BrMetaBlock> hm(n_mbs);
-    CK(cudaMemcpyAsync(hm.data(), mbs, n_mbs * sizeof(BrMetaBlock), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(hm.data(), s.mbs, n_mbs * sizeof(BrMetaBlock), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    std::vector<u64> h_soff(n_mbs), h_ooff(n_mbs);
-    size_t scratch_total = 0, outw_total = 0;
-    for (u32 i = 0; i < n_mbs; ++i) {
-      h_soff[i] = scratch_total; h_ooff[i] = outw_total;
-      if (hm[i].compress) {
-        scratch_total += ((size_t)br_mb_scratch_bytes(P, hm[i].nlit, hm[i].ncmd) + 255) & ~(size_t)255;
-        outw_total += (2 * (size_t)(hm[i].end - hm[i].start) + 503) / 4 + 16;
-      }
-    }
-    size_t out_cap = (size_t)n + ((size_t)n >> 3) + 4096 + 8ull * n_mbs;
+    BrMbLayout L;
+    br_mb_layout(P, hm.data(), n_mbs, L);
     const size_t C = total_cmds;
-    size_t need2 = scratch_total + outw_total * 4 + out_cap + (C + 2) * (sizeof(BrCmd) + 26) + ((size_t)n + 8) * 12 +
-                   scan_tmp_words((size_t)n + C + 8) * 4 * 2 + n_mbs * (32 + sizeof(BrCopyDesc) + sizeof(BrMbAux)) + (1 << 16);
-    if (!job->arena2.reserve(need2)) return 0;
-    BrArena& B = job->arena2;
-    u8* scratch = B.take<u8>(scratch_total + 256); u32* outbits = B.take<u32>(outw_total + 64);
-    u32* out = B.take<u32>(out_cap / 4 + 16); BrCmd* cmds_all = B.take<BrCmd>(C + 1);
-    u64* d_soff = B.take<u64>(n_mbs); u64* d_ooff = B.take<u64>(n_mbs);
-    BrCopyDesc* desc = B.take<BrCopyDesc>(n_mbs); u32* res = B.take<u32>(16);
-    u32* lit_ord = B.take<u32>(C + 2); u32* cmd_pos = B.take<u32>(C + 2); u32* dist_ord = B.take<u32>(C + 2);
-    u32* cmd_len = B.take<u32>(C + 2); u32* lit_bit_base = B.take<u32>(C + 2); u32* cmd_mb = B.take<u32>(C + 2);
-    u16* dist_sym = B.take<u16>(C + 2);
-    u32* lit_pos = B.take<u32>((size_t)n + 2); u32* lit_cmd = B.take<u32>((size_t)n + 2); u32* lit_len = B.take<u32>((size_t)n + 2);
-    BrMbAux* aux = B.take<BrMbAux>(n_mbs);
-    u32* stmp = B.take<u32>(scan_tmp_words((size_t)n + C + 8) * 2);
-    if (!stmp) return 0;
-    CK(cudaMemcpyAsync(d_soff, h_soff.data(), n_mbs * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_ooff, h_ooff.data(), n_mbs * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(outbits, 0, (outw_total + 64) * 4, st));
-    CK(cudaMemsetAsync(out, 0, out_cap + 64, st));
-    k_compact<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s, cmds_all, block_mb);
+    BrEnt e; memset(&e, 0, sizeof(e));
+    BrCmd* cmds_all; u64 *soff, *ooff; BrCopyDesc* desc; u32 *out, *res, *lit_ord, *cmd_pos, *dist_ord, *stmp;
+    auto carve2 = [&](BrCarve& B) {
+      e.scratch = B.take<u8>(L.scratch_bytes + 256); e.outbits = B.take<u32>(L.out_words + 64);
+      out = B.take<u32>(L.out_cap / 4 + 16); e.cmds = cmds_all = B.take<BrCmd>(C + 1);
+      e.scratch_off = soff = B.take<u64>(n_mbs); e.out_off = ooff = B.take<u64>(n_mbs);
+      desc = B.take<BrCopyDesc>(n_mbs); res = B.take<u32>(16);
+      e.lit_ord = lit_ord = B.take<u32>(C + 2); e.cmd_pos = cmd_pos = B.take<u32>(C + 2); e.dist_ord = dist_ord = B.take<u32>(C + 2);
+      e.cmd_len = B.take<u32>(C + 2); e.lit_bit_base = B.take<u32>(C + 2); e.cmd_mb = B.take<u32>(C + 2);
+      e.dist_sym = B.take<u16>(C + 2);
+      e.lit_pos = B.take<u32>((size_t)n + 2); e.lit_cmd = B.take<u32>((size_t)n + 2); e.lit_len = B.take<u32>((size_t)n + 2);
+      e.aux = B.take<BrMbAux>(n_mbs);
+      stmp = B.take<u32>(scan_tmp_words((size_t)n + C + 8) * 2);
+    };
+    if (!br_carve(job->arena2, carve2)) return 0;
+    CK(cudaMemcpyAsync(soff, L.scratch_off.data(), n_mbs * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ooff, L.out_off.data(), n_mbs * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(e.outbits, 0, (L.out_words + 64) * 4, st));
+    CK(cudaMemsetAsync(out, 0, L.out_cap + 64, st));
+    k_compact<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s, cmds_all, s.block_mb);
     cudaEventRecord(ev[8], st);
     // E0: ordinals
     k_cmd_scan_inputs<<<(u32)((C + 1 + 255) / 256), 256, 0, st>>>(cmds_all, (u32)C, lit_ord, cmd_pos, dist_ord);
@@ -890,14 +798,10 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
     CK(cudaMemcpyAsync(hp + 24, lit_ord + C, 4, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(hp + 25, dist_ord + C, 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    BrEnt e; memset(&e, 0, sizeof(e));
-    e.cmds = cmds_all; e.total_cmds = (u32)C; e.total_lits = hp[24]; e.total_dist = hp[25];
-    e.lit_ord = lit_ord; e.cmd_pos = cmd_pos; e.dist_ord = dist_ord; e.lit_pos = lit_pos; e.lit_cmd = lit_cmd;
-    e.dist_sym = dist_sym; e.lit_len = lit_len; e.cmd_len = cmd_len; e.lit_bit_base = lit_bit_base; e.cmd_mb = cmd_mb;
-    e.aux = aux; e.scratch = scratch; e.scratch_off = d_soff; e.outbits = outbits; e.out_off = d_ooff;
+    e.total_cmds = (u32)C; e.total_lits = hp[24]; e.total_dist = hp[25];
     if (e.total_lits > n) return 0;
     const u32 grid_mbs = n_mbs < 65535u ? n_mbs : 65535u;
-    k_cmd_mb<<<dim3(64, grid_mbs), 256, 0, st>>>(s, cmd_mb, n_mbs);
+    k_cmd_mb<<<dim3(64, grid_mbs), 256, 0, st>>>(s, e.cmd_mb, n_mbs);
     k_expand<<<(u32)((C + 127) / 128 + 1), 128, 0, st>>>(e);
     k_mb_setup<<<n_mbs, 32, 0, st>>>(s, e);
     if (P.mb_kind) k_prep_flat<<<n_mbs, 64, 0, st>>>(s, e);   // qualities 2, 3: no block split, one code per category
@@ -909,22 +813,22 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
     }
     k_lit_bits<<<(e.total_lits + 1 + 255) / 256, 256, 0, st>>>(s, e);
     k_cmd_bits<<<(u32)((C + 1 + 255) / 256), 256, 0, st>>>(s, e);
-    scan_exclusive(lit_len, e.total_lits + 1, stmp, st);
-    scan_exclusive(cmd_len, (u32)C + 1, stmp, st);
+    scan_exclusive(e.lit_len, e.total_lits + 1, stmp, st);
+    scan_exclusive(e.cmd_len, (u32)C + 1, stmp, st);
     k_emit_cmd<<<(u32)((C + 255) / 256), 256, 0, st>>>(s, e);
     if (e.total_lits) k_emit_lit<<<(e.total_lits + 255) / 256, 256, 0, st>>>(s, e);
     cudaEventRecord(ev[9], st);
     cudaEventRecord(ev[3], st);
     ++job->stats.encode_launches; job->stats.launches += 24;
-    k_assemble_scan<<<1, 32, 0, st>>>(s, d_ooff, out, desc, res, with_header, d_cut_kind, d_cut_end, d_stream_end);
+    k_assemble_scan<<<1, 32, 0, st>>>(s, ooff, out, desc, res, plan.with_header, cut_kind, cut_end, stream_end);
     CK(cudaMemcpyAsync(hp + 16, res, 16, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     if (hp[18]) {   // encode.c:604: a coded metablock is larger than its input -> it is stored raw (br_assemble_scan marked
                     // it in force_unc) and the parse behind it is redone with the restored distance cache
-      if (rounds > (int)nblk + 8) return 0;   // (every round stores at least one more metablock raw)
+      if (rounds > (int)plan.max_rounds) return 0;
       continue;
     }
-    k_assemble_copy<<<dim3(64, grid_mbs), 256, 0, st>>>(s, desc, outbits, out, n_mbs);
+    k_assemble_copy<<<dim3(64, grid_mbs), 256, 0, st>>>(s, desc, e.outbits, out, n_mbs);
     final_out = (const u8*)out; final_size = ((u64)hp[17] << 32) | hp[16];
     break;
   }
@@ -942,11 +846,11 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
   job->stats.nblocks = nb; job->stats.n_metablocks = n_mbs; job->stats.rounds = (u32)rounds;
   job->stats.out_bytes = final_size; job->stats.in_bytes = n;
   if (cuts && cuts->end_bit && ncuts && nstreams == 1) {
-    CK(cudaMemcpyAsync(cuts->end_bit, d_cut_end, ncuts * 8ull, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(cuts->end_bit, cut_end, ncuts * 8ull, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
   if (cuts && cuts->stream_end && nstreams > 1) {
-    CK(cudaMemcpyAsync(cuts->stream_end, d_stream_end, nstreams * 8ull, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(cuts->stream_end, stream_end, nstreams * 8ull, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
   *d_out = final_out; *out_size = final_size;
@@ -991,25 +895,16 @@ extern "C" __attribute__((visibility("default"))) int br_debug_index(int quality
                                                                     u32* h_seg, u32* h_rank, u32* h_keys) {
   BrParams P;
   if (n == 0 || !br_derive_params(quality, lgwin, n, n, &P)) return 0;
-  const u32 ntiles = (n + RADIX_TILE - 1) / RADIX_TILE;
   BrBlk B; memset(&B, 0, sizeof(B)); B.start = 0; B.end = n; B.base = 0; B.send = n;
-  size_t need = 0;
-  auto add = [&](size_t bytes) { need += (bytes + 255) & ~(size_t)255; };
-  add((size_t)n + 64); add(sizeof(BrBlk)); add(4ull * n + 16); add(4ull * n + 16); add(4ull * n + 16); add(4ull * n + 16);
-  add(4ull * n + 16); add(4ull * n + 16); add(4ull * n + 16); add(4ull * n + 16); add(4ull * n + 16); add((P.nbuckets + 4) * 4ull);
-  add(1024ull * ntiles); add(scan_tmp_words(256ull * ntiles) * 4);
+  u8* data; BrBlk* blk; BrIndexBufs b;
+  auto carve = [&](BrCarve& A) {
+    data = A.take<u8>((size_t)n + 64); blk = A.take<BrBlk>(1);
+    carve_index(A, P, b); carve_index_quick(A, P, b);
+  };
   BrArena A;
-  if (!A.reserve(need)) return 0;
-  u8* data = A.take<u8>((size_t)n + 64); BrBlk* blk = A.take<BrBlk>(1);
-  BrIndexBufs b;
-  b.K1 = A.take<u16>((size_t)n + 8); b.K2 = A.take<u16>((size_t)n + 8); b.V1 = A.take<u32>((size_t)n + 4);
-  b.S = A.take<u32>((size_t)n + 4); b.rank = A.take<u32>((size_t)n + 4);
-  b.qk_keys = A.take<u32>((size_t)n + 4); b.qk_K1 = A.take<u32>((size_t)n + 4); b.qk_V1 = A.take<u32>((size_t)n + 4);
-  b.qk_V2 = A.take<u32>((size_t)n + 4); b.seg = A.take<u32>(P.nbuckets + 4);
-  b.hist = A.take<u32>(256ull * ntiles); b.scan_tmp = A.take<u32>(scan_tmp_words(256ull * ntiles));
+  if (!br_carve(A, carve)) return 0;
   int ok = 0;
   std::vector<u16> k16;
-  if (!b.scan_tmp) goto done;
   if (cudaMemset(data, 0, (size_t)n + 64) != cudaSuccess || cudaMemcpy(data, h_in, n, cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy(blk, &B, sizeof(BrBlk), cudaMemcpyHostToDevice) != cudaSuccess) goto done;
   br_build_index(P, data, blk, 1, b, 0);
@@ -1053,83 +948,59 @@ extern "C" __attribute__((visibility("default"))) int br_debug_search(
     int quality, int lgwin, int lgblock, u32 size_hint, const u8* h_in, u32 n, const u32* h_bounds, u32 nstreams,
     const u32* h_snap, const u32* h_own, u32 heavy_min, const u32* h_probes, u32 np, u32* h_res, u16* h_tagS,
     u32* h_storedS, u32* h_prefS) {
-  BrParams P;
-  if (n == 0 || nstreams == 0 || h_bounds[nstreams - 1] != n || !br_derive_params(quality, lgwin, size_hint, n, &P, lgblock)) return 0;
-  if (heavy_min) P.heavy_min = heavy_min;
-  if (nstreams > 1) P.multi = nstreams;
+  if (nstreams == 0 || h_bounds[nstreams - 1] != n) return 0;
   std::vector<u32> kinds(nstreams, 3);
-  std::vector<BrBlk> hblk;
-  u32 nb = 0;
-  br_build_blocks(P, n, h_bounds, nstreams - 1, true, nullptr, hblk, &nb, kinds.data());
-  const u32 nblk = (u32)hblk.size();
-  std::vector<u32> h_slot(((size_t)n >> P.lgblock) + 2, 0);
-  { u32 b = 0; for (size_t i = 0; i < h_slot.size(); ++i) { const u64 p = (u64)i << P.lgblock; while (b + 1 < nblk && hblk[b].end <= p) ++b; h_slot[i] = b; } }
+  const BrCuts cuts = {h_bounds, kinds.data(), nstreams - 1, 1, 1, 0, nullptr, lgblock, 0, 0, nullptr};
+  const BrSchedKnobs knobs = {BR_KNOB_KEEP, BR_KNOB_KEEP, BR_KNOB_KEEP, heavy_min ? heavy_min : BR_KNOB_KEEP, BR_KNOB_KEEP,
+                              BR_KNOB_KEEP};
+  BrStreamPlan plan;
+  if (!br_plan_stream(quality, lgwin, size_hint, n, &cuts, &knobs, &plan)) return 0;
   BrDeviceTables* T = get_tables();
   if (!T) return 0;
-  const int G[3] = {P.quick ? 0 : P.block_bits >= 6 ? BR_WALK_G_DEEP : BR_WALK_G_SMALL, 1, 8};
-  const int nvar = !P.quick && P.block_bits >= 6 ? 3 : 1;
-  const u32 ntiles = (n + RADIX_TILE - 1) / RADIX_TILE, nwords = (n + 31) / 32 + 2, nsnap = (n + 1023) / 1024;
+  const BrParams& P = plan.P;
+  const int nvar = !P.quick && P.quality >= 7 ? 3 : 1;
+  const u32 nblk = (u32)plan.blk.size(), nwords = (n + 31) / 32 + 2, nsnap = (n + 1023) / 1024;
   const size_t nsaw = P.quick ? ((size_t)n << P.qk_sweep_bits) + 16 : 16;
-  size_t need = 1 << 16;
-  auto add = [&](size_t bytes) { need += (bytes + 255) & ~(size_t)255; };
-  add((size_t)n + 64); add(nblk * sizeof(BrBlk)); add(h_slot.size() * 4);
-  for (int i = 0; i < 9; ++i) add(4ull * n + 16);
-  add((P.nbuckets + 4) * 4ull); add(1024ull * ntiles); add(scan_tmp_words(256ull * ntiles) * 4);
-  add(2ull * n + 16); add(nwords * 4ull * 3 + 256); add(((size_t)n / 1024 + 8) * 8); add(scan_tmp_words((size_t)n / 1024 + 8) * 4);
-  add(nsaw * 8); add((size_t)np * BR_PROBE_WORDS * 4 * (1 + nvar));
-  BrArena A;
-  if (!A.reserve(need)) return 0;
-  u8* data = A.take<u8>((size_t)n + 64); BrBlk* blk = A.take<BrBlk>(nblk); u32* slot_blk = A.take<u32>(h_slot.size());
-  BrIndexBufs b;
-  b.K1 = A.take<u16>((size_t)n + 8); b.K2 = A.take<u16>((size_t)n + 8); b.V1 = A.take<u32>((size_t)n + 4);
-  b.S = A.take<u32>((size_t)n + 4); b.rank = A.take<u32>((size_t)n + 4);
-  b.qk_keys = A.take<u32>((size_t)n + 4); b.qk_K1 = A.take<u32>((size_t)n + 4); b.qk_V1 = A.take<u32>((size_t)n + 4);
-  b.qk_V2 = A.take<u32>((size_t)n + 4); b.seg = A.take<u32>(P.nbuckets + 4);
-  b.hist = A.take<u32>(256ull * ntiles); b.scan_tmp = A.take<u32>(scan_tmp_words(256ull * ntiles));
-  u16* tagS = A.take<u16>((size_t)n + 8);
-  u32* snap = A.take<u32>(nwords); u32* own = A.take<u32>(nwords); u32* storedS = A.take<u32>(nwords + 64);
-  u32* prefS = A.take<u32>((size_t)n / 1024 + 8); u32* cntS = A.take<u32>((size_t)n / 1024 + 8);
-  u32* scan_tmp2 = A.take<u32>(scan_tmp_words((size_t)n / 1024 + 8));
-  u32* qpred = A.take<u32>(nsaw); u32* saw = A.take<u32>(nsaw);
-  u32* probes = A.take<u32>((size_t)np * BR_PROBE_WORDS); u32* res = A.take<u32>((size_t)np * BR_PROBE_WORDS * nvar);
   BrStream s; memset(&s, 0, sizeof(s));
+  s.P = P; s.nblk = nblk; s.bits_words = nwords;
+  BrIndexBufs b;
+  u8* data; u32 *snap, *own, *storedS, *prefS, *cntS, *scan_tmp2, *qpred, *probes, *res;
+  auto carve = [&](BrCarve& A) {
+    s.data = data = A.take<u8>((size_t)n + 64); s.blk = A.take<BrBlk>(nblk); s.slot_blk = A.take<u32>(plan.slot_blk.size());
+    carve_index(A, P, b); carve_index_quick(A, P, b);
+    s.bits_latest = snap = A.take<u32>(nwords); own = A.take<u32>(nwords); s.storedS = storedS = A.take<u32>(nwords + 64);
+    s.prefS = prefS = A.take<u32>((size_t)n / 1024 + 8); cntS = A.take<u32>((size_t)n / 1024 + 8);
+    scan_tmp2 = A.take<u32>(scan_tmp_words((size_t)n / 1024 + 8));
+    s.qpred = qpred = A.take<u32>(nsaw); s.saw = A.take<u32>(nsaw);
+    probes = A.take<u32>((size_t)np * BR_PROBE_WORDS); res = A.take<u32>((size_t)np * BR_PROBE_WORDS * nvar);
+  };
+  auto probe = [&](auto g, int v) {
+    k_search_probe<decltype(g)::value><<<(np + 3) / 4, 128>>>(s, own, probes, np, res + (size_t)v * np * BR_PROBE_WORDS);
+  };
+  BrArena A;
+  if (!br_carve(A, carve)) return 0;
+  s.S = b.S; s.rank = b.rank; s.seg = b.seg; s.skeys = b.K2; s.tagS = b.tagS;
+  br_bind_tables(s, T->blob, T->log2tab, T->log2tab_n);
   int ok = 0;
-  if (!res) goto done;
-  s.P = P; s.data = data; s.S = b.S; s.rank = b.rank; s.seg = b.seg; s.skeys = b.K2; s.tagS = tagS;
-  s.bits_latest = snap; s.bits_words = nwords; s.storedS = storedS; s.prefS = prefS;
-  s.blk = blk; s.nblk = nblk; s.slot_blk = slot_blk; s.qpred = qpred; s.saw = saw;
-  { const u8* p = T->blob + 8;
-    s.dict_size_bits = p; p += 32; s.dict_offsets = (const u32*)p; p += 128; s.dict = p; p += 122784;
-    s.dict_hash_words = (const u16*)p; p += 65536; s.dict_hash_lengths = p; p += 32768; s.ctx_lut = p; }
-  s.log2tab = T->log2tab; s.log2tab_n = T->log2tab_n;
   if (cudaMemset(data, 0, (size_t)n + 64) != cudaSuccess || cudaMemcpy(data, h_in, n, cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(blk, hblk.data(), nblk * sizeof(BrBlk), cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(slot_blk, h_slot.data(), h_slot.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(s.blk, plan.blk.data(), nblk * sizeof(BrBlk), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy((u32*)s.slot_blk, plan.slot_blk.data(), plan.slot_blk.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemset(snap, 0, nwords * 4ull) != cudaSuccess || cudaMemset(own, 0, nwords * 4ull) != cudaSuccess ||
       cudaMemcpy(snap, h_snap, (n + 31) / 32 * 4ull, cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy(own, h_own, (n + 31) / 32 * 4ull, cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemset(saw, 0xEE, nsaw * 4) != cudaSuccess ||
+      cudaMemset(s.saw, 0xEE, nsaw * 4) != cudaSuccess ||
       cudaMemcpy(probes, h_probes, (size_t)np * BR_PROBE_WORDS * 4, cudaMemcpyHostToDevice) != cudaSuccess) goto done;
-  br_build_index(P, data, blk, nblk, b, 0);
+  br_build_index(P, data, s.blk, nblk, b, 0);
   if (P.quick) k_slot_pred<<<nblk, 256, 0>>>(s, qpred);
-  k_tags<<<(n + 255) / 256, 256>>>(data, b.S, n, tagS);
+  k_tags<<<(n + 255) / 256, 256>>>(data, b.S, n, b.tagS);
   k_build_storedS<<<nsnap, 1024>>>(s, storedS, cntS);
   if (cudaMemcpy(prefS, cntS, nsnap * 4ull, cudaMemcpyDeviceToDevice) != cudaSuccess) goto done;
   scan_exclusive(prefS, nsnap, scan_tmp2, 0);
-  for (int v = 0; v < nvar; ++v) {
-    u32* r = res + (size_t)v * np * BR_PROBE_WORDS;
-    const u32 grid = (np + 3) / 4;
-    switch (G[v]) {
-      case 0: k_search_probe<0><<<grid, 128>>>(s, own, probes, np, r); break;
-      case 1: k_search_probe<1><<<grid, 128>>>(s, own, probes, np, r); break;
-      case 4: k_search_probe<4><<<grid, 128>>>(s, own, probes, np, r); break;
-      case 8: k_search_probe<8><<<grid, 128>>>(s, own, probes, np, r); break;
-      default: goto done;
-    }
-  }
+  br_walk_dispatch(P, [&](auto g, auto) { probe(g, 0); });
+  if (nvar == 3) { probe(std::integral_constant<int, 1>(), 1); probe(std::integral_constant<int, 8>(), 2); }
   if (cudaDeviceSynchronize() != cudaSuccess ||
       cudaMemcpy(h_res, res, (size_t)np * BR_PROBE_WORDS * 4 * nvar, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
-  if (h_tagS && cudaMemcpy(h_tagS, tagS, 2ull * n, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  if (h_tagS && cudaMemcpy(h_tagS, b.tagS, 2ull * n, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
   if (h_storedS && cudaMemcpy(h_storedS, storedS, (n + 31) / 32 * 4ull, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
   if (h_prefS && cudaMemcpy(h_prefS, prefS, nsnap * 4ull, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
   ok = nvar;

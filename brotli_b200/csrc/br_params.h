@@ -1,9 +1,11 @@
 // br_params.h -- host-side parameter derivation: what SanitizeParams / ComputeLgBlock /
 // ChooseHasher / ComputeRbBits / MaxMetablockSize (c/enc/quality.h:59-225) decide for a
-// given (quality, lgwin, size_hint).  Host only.
+// given (quality, lgwin, size_hint), and the plan of one stream built from them.  Host only.
 #pragma once
+#include <type_traits>
 #include <vector>
 #include "br_types.h"
+#include "br_pipeline.h"
 
 // Returns 0 if the combination is outside what this library implements (the BrotliEncoder*
 // entry points then fail instead of silently doing something else).
@@ -112,4 +114,117 @@ static inline void br_build_blocks(const BrParams& P, u32 n, const u32* cuts, u3
   }
   { u32 send = n; for (size_t i = blks.size(); i-- > 0;) { if (blks[i].is_last) send = blks[i].end; blks[i].send = send; } }
   if (nchunks_total) *nchunks_total = total;
+}
+
+// Everything the host decides about one stream (or batch of streams) before its first kernel runs.
+struct BrStreamPlan {
+  BrParams P;                    // with the cuts, the knobs, the batch rules, finish_empty, nblocks and max_epochs applied
+  std::vector<BrBlk> blk;        // the input blocks (br_build_blocks)
+  std::vector<u32> slot_blk;     // BrStream::slot_blk
+  std::vector<u32> stream_blk;   // BrStream::stream_blk: [nstreams + 1], the first input block of every stream
+  u32 nstreams;
+  u32 cmd_stride;                // commands one chunk may emit (BrStream::cmd_stride)
+  u32 ran_cap;                   // entries of ran_list
+  u32 max_rounds;                // late-fallback rounds after which the stream fails
+  bool is_final;
+  int with_header;
+};
+
+// Plans a stream of n bytes: false where the combination is outside what the pipeline implements.  cuts, knobs (nullable):
+// br_pipeline.h.  batch_chunk_bits (the sim's schedules): the chunk size of a batch of streams instead of
+// br_batch_chunk_bits.  chunks (nullable): also the chunk table (the CUDA pipeline builds it on the device, k_build_chunks).
+static inline bool br_plan_stream(int quality, int lgwin, u32 size_hint, u32 n, const BrCuts* cuts, const BrSchedKnobs* knobs,
+                                  BrStreamPlan* plan, u32 batch_chunk_bits = BR_KNOB_KEEP,
+                                  std::vector<BrBlockIn>* chunks = nullptr) {
+  BrParams& P = plan->P;
+  if (n == 0 || !br_derive_params(quality, lgwin, size_hint, n, &P, cuts ? cuts->lgblock : 0)) return false;
+  P.disable_ctx = cuts && cuts->disable_ctx ? 1u : 0u;
+  P.stream_offset = cuts ? (cuts->stream_offset < P.max_backward ? cuts->stream_offset : P.max_backward) : 0u;   // encode.c:680
+  if (knobs) {
+    if (knobs->sweep_epoch != BR_KNOB_KEEP) P.sweep_epoch = knobs->sweep_epoch;
+    if (knobs->force_epoch != BR_KNOB_KEEP) P.force_epoch = knobs->force_epoch;
+    if (knobs->step_cap != BR_KNOB_KEEP) P.step_cap = knobs->step_cap;
+    if (knobs->heavy_min != BR_KNOB_KEEP) P.heavy_min = knobs->heavy_min;
+    if (knobs->pilot != BR_KNOB_KEEP) P.pilot = knobs->pilot;
+    if (knobs->sweep_blocks != BR_KNOB_KEEP) {
+      if (knobs->sweep_blocks == 0 || (knobs->sweep_blocks & (knobs->sweep_blocks - 1))) return false;   // (a power of two)
+      P.sweep_blocks = knobs->sweep_blocks;
+    }
+  }
+  const u32 ncuts = cuts ? cuts->n : 0;
+  u32 nstreams = 1;
+  for (u32 i = 0; i < ncuts; ++i) if (cuts->kind[i] == 3) ++nstreams;
+  if (nstreams > 1) {
+    // a batch of independent streams (each below BR_SMALL_STREAM, size_hint = the largest): no FLUSH cuts, all finished
+    if (nstreams != ncuts + 1 || !cuts->is_final || !cuts->with_header || cuts->finish_empty || cuts->stream_offset ||
+        cuts->pos[ncuts - 1] >= n || size_hint >= BR_SMALL_STREAM) return false;
+    P.multi = nstreams; P.pilot = 0;
+    P.chunk_bits = batch_chunk_bits != BR_KNOB_KEEP ? batch_chunk_bits : br_batch_chunk_bits(n);
+  }
+  if (P.quick && P.stream_offset) return false;   // (STREAM_OFFSET: quality 5..9)
+  plan->is_final = cuts ? cuts->is_final != 0 : true;
+  plan->with_header = cuts ? cuts->with_header : 1;
+  P.finish_empty = cuts && cuts->finish_empty ? 1u : 0u;
+  if (!plan->is_final && (ncuts == 0 || cuts->pos[ncuts - 1] != n)) return false;   // an unfinished stream ends at a cut
+  if (P.finish_empty && (!plan->is_final || (ncuts && cuts->pos[ncuts - 1] == n))) return false;
+  std::vector<BrBlk>& blk = plan->blk;
+  blk.clear();
+  if (chunks) chunks->clear();
+  u32 nb = 0;
+  br_build_blocks(P, n, cuts ? cuts->pos : nullptr, ncuts, plan->is_final && !P.finish_empty, chunks, blk, &nb,
+                  cuts ? cuts->kind : nullptr);
+  const u32 nblk = (u32)blk.size();
+  plan->slot_blk.assign(((size_t)n >> P.lgblock) + 2, 0);
+  for (size_t i = 0, b = 0; i < plan->slot_blk.size(); ++i) {
+    while (b + 1 < nblk && blk[b].end <= ((u64)i << P.lgblock)) ++b;
+    plan->slot_blk[i] = (u32)b;
+  }
+  plan->stream_blk.assign(nstreams + 1, nblk);
+  for (u32 bi = nblk; bi-- > 0;) plan->stream_blk[blk[bi].stream] = bi;
+  plan->nstreams = nstreams;
+  P.nblocks = nb;
+  // Launch bound: in forced mode every launch finalises at least one input block (at most two launches per block with
+  // the conservative block-level re-marks), and a late uncompressed fallback restarts the count at most once per metablock.
+  P.max_epochs = 4 * nb + 4096;
+  plan->cmd_stride = (1u << P.chunk_bits) / 2 + 2;
+  // ran_list: every chunk is walked at most once per launch -- by its own scheduled walker or by the one sweep that chases
+  // into it, and in a forced launch the walkers scheduled behind the forced one in its input block stand down
+  // (br_walk_block) -- so a launch appends at most nb entries
+  plan->ran_cap = nb + 16;
+  plan->max_rounds = nblk + 8;   // (every round stores at least one more metablock raw)
+  return true;
+}
+
+// Points s at the constant tables: brotli_tables.bin (oracle/gen_tables.c) at `blob` and the log2 table.
+static inline void br_bind_tables(BrStream& s, const u8* blob, const double* log2tab, u32 log2tab_n) {
+  const u8* p = blob + 8;
+  s.dict_size_bits = p; p += 32;
+  s.dict_offsets = (const u32*)p; p += 128;
+  s.dict = p; p += 122784;
+  s.dict_hash_words = (const u16*)p; p += 65536;
+  s.dict_hash_lengths = p; p += 32768;
+  s.ctx_lut = p;
+  s.log2tab = log2tab; s.log2tab_n = log2tab_n;
+}
+
+// G = bucket-ring rows the walker fetches together (br_lz77.h): 1 for the 16/32-entry rings of quality 5-6 (throughput
+// bound, 8 CTAs per SM), 4 for the 64-256-entry rings of quality 7-9 (more registers, fewer resident warps).
+#ifndef BR_WALK_G_DEEP
+#define BR_WALK_G_DEEP 4    /* rows fetched together for the 256-entry rings of quality 9: 8 (the whole ring, 125 registers,
+                               16 warps per SM) walks one chunk faster, 4 (96 registers, 20 warps per SM) won on the whole
+                               job of config C4 when the two were timed against each other */
+#endif
+#ifndef BR_WALK_G_SMALL
+#define BR_WALK_G_SMALL 1   /* rows fetched together for the 16/32-entry rings */
+#endif
+// Calls f(G, M) with the walker's template arguments for P as std::integral_constants: G the row grouping (0: the quick
+// search of qualities 2..4), M a batch of streams.
+template <int G, class F> static inline void br_walk_dispatch_m(const BrParams& P, F& f) {
+  if (P.multi) f(std::integral_constant<int, G>(), std::true_type());
+  else f(std::integral_constant<int, G>(), std::false_type());
+}
+template <class F> static inline void br_walk_dispatch(const BrParams& P, F&& f) {
+  if (P.quick) br_walk_dispatch_m<0>(P, f);
+  else if (P.block_bits >= 6) br_walk_dispatch_m<BR_WALK_G_DEEP>(P, f);
+  else br_walk_dispatch_m<BR_WALK_G_SMALL>(P, f);
 }

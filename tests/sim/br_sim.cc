@@ -36,12 +36,11 @@ extern "C" int sim_init(const u8* blob, size_t len, u32 log2n) {
 
 // An explicit schedule of the LZ77 fixpoint (sim_compress_sched): the knobs of BrParams that decide which chunks a launch
 // walks and when the safety nets take over, and the order in which the sim runs a launch's walks and commits (on the GPU
-// they run concurrently, in no fixed order).  SIM_KEEP keeps the value br_derive_params chose.
-#define SIM_KEEP 0xffffffffu
+// they run concurrently, in no fixed order).  BR_KNOB_KEEP keeps the value the plan chose.
 enum { SIM_ORDER_SCHEDULED = 0, SIM_ORDER_REVERSED = 1, SIM_ORDER_SHUFFLED = 2 };
 struct SimSched {
-  u32 sweep_epoch, force_epoch, step_cap, heavy_min, pilot, sweep_blocks;
-  u32 batch_chunk_bits;             // chunk size of a batch of streams (log2)
+  BrSchedKnobs knobs;               // as br_debug_compress_sched takes them (br_pipeline.h)
+  u32 batch_chunk_bits;             // chunk size of a batch of streams (log2; br_plan_stream)
   u32 walk_order, commit_order;     // SIM_ORDER_*; commit_order applies to the br_cover_run and the br_commit_bits loops
   u32 walk_seed, commit_seed;       // SIM_ORDER_SHUFFLED
   u32 verify;                       // != 0: re-walk every chunk at the fixpoint (SIM_ST_VERIFY_DIFF); the output is unchanged
@@ -55,7 +54,7 @@ enum {
   SIM_ST_PREDICT_OK = 8,        // block boundaries a sweep crossed (br_predict_next_block true; BR_SIM_DEBUG builds only)
   SIM_ST_PREDICT_NO = 9,        // block boundaries where the prediction refused (BR_SIM_DEBUG builds only)
   SIM_ST_MAX_WALKS = 10,        // the largest number of chunk walks of one launch (counters[4])
-  SIM_ST_RAN_CAP = 11,          // capacity of ran_list, as the product sizes it
+  SIM_ST_RAN_CAP = 11,          // capacity of ran_list (BrStreamPlan::ran_cap)
   SIM_ST_VERIFY_DIFF = 12,      // chunks whose re-walk at the fixpoint gives other bits or another out-state (SimSched::verify)
   SIM_ST_WORDS = 16
 };
@@ -73,16 +72,15 @@ struct SimStream {
   std::vector<BrBlockOut> bout;
   std::vector<BrCmd> cmd_blocks, cmds_all;
   std::vector<BrMetaBlock> mbs;
-  std::vector<BrBlk> blks;
+  BrStreamPlan plan;                // the block, slot and stream tables and the sizes, as the product plans them
   std::vector<BrBlkIn> blkin;
   std::vector<u32> key_flips, saw, qpred;
-  std::vector<u32> dirty_list, ran_list, slot_blk, stream_blk, stream_nmb, stream_ncmd;
+  std::vector<u32> dirty_list, ran_list, stream_nmb, stream_ncmd;
   std::vector<BrMetaBlock> mbs_stage;
   int iterations = 0;
   u64 block_runs = 0;
   double model_cost = 0;
   SimSched sched;
-  u32 ran_cap = 0;
   u32 st[SIM_ST_WORDS] = {};
 };
 
@@ -118,75 +116,51 @@ static void sim_build_storedS(SimStream& m) {
   }
 }
 
-struct SimCuts { const u32* pos; const u32* kind; u32 n; int is_final; int with_header; int finish_empty; u64* end_bit; u32 size_hint; int lgblock; int disable_ctx; u32 stream_offset; u64* stream_end; };
-// the schedule of the tools' environment switches (BR_SIM_*): everything else as derived, walks and commits in list order
+// the schedule of the tools' environment switches (BR_SIM_*): everything else as planned, walks and commits in list order
 static SimSched sim_sched_from_env() {
   SimSched c;
-  auto env = [](const char* name) { const char* v = getenv(name); return v ? (u32)atoi(v) : SIM_KEEP; };
-  c.heavy_min = env("BR_SIM_HEAVY_MIN"); c.step_cap = env("BR_SIM_STEP_CAP"); c.sweep_epoch = env("BR_SIM_SWEEP_EPOCH");
-  c.sweep_blocks = env("BR_SIM_SWEEP_BLOCKS"); c.pilot = env("BR_SIM_PILOT"); c.force_epoch = env("BR_SIM_FORCE_EPOCH");
+  auto env = [](const char* name) { const char* v = getenv(name); return v ? (u32)atoi(v) : BR_KNOB_KEEP; };
+  c.knobs.heavy_min = env("BR_SIM_HEAVY_MIN"); c.knobs.step_cap = env("BR_SIM_STEP_CAP"); c.knobs.sweep_epoch = env("BR_SIM_SWEEP_EPOCH");
+  c.knobs.sweep_blocks = env("BR_SIM_SWEEP_BLOCKS"); c.knobs.pilot = env("BR_SIM_PILOT"); c.knobs.force_epoch = env("BR_SIM_FORCE_EPOCH");
   c.batch_chunk_bits = env("BR_SIM_BATCH_CHUNK_BITS");
   c.walk_order = c.commit_order = SIM_ORDER_SCHEDULED; c.walk_seed = c.commit_seed = 0;
   c.verify = getenv("BR_SIM_VERIFY") ? 1u : 0u;
   return c;
 }
 
-static SimStream* sim_setup(int q, int lgwin, const u8* in, u32 n, const SimCuts* cuts = nullptr, const SimSched* sched = nullptr) {
+// The stream planned by br_plan_stream (nullptr where the product refuses it), with the sim's own memory.
+static SimStream* sim_setup(int q, int lgwin, u32 size_hint, const u8* in, u32 n, const BrCuts* cuts = nullptr,
+                            const SimSched* sched = nullptr) {
   SimStream* m = new SimStream();
+  m->sched = sched ? *sched : sim_sched_from_env();
+  BrStreamPlan& plan = m->plan;
+  if (!br_plan_stream(q, lgwin, size_hint, n, cuts, &m->sched.knobs, &plan, m->sched.batch_chunk_bits, &m->bin)) {
+    delete m; return nullptr;
+  }
   BrStream& s = m->s;
   memset(&s, 0, sizeof(s));
-  if (!br_derive_params(q, lgwin, cuts ? cuts->size_hint : n, n, &s.P, cuts ? cuts->lgblock : 0)) { delete m; return nullptr; }
-  s.P.disable_ctx = cuts && cuts->disable_ctx ? 1u : 0u;
-  s.P.stream_offset = cuts ? (cuts->stream_offset < s.P.max_backward ? cuts->stream_offset : s.P.max_backward) : 0u;
-  BrParams& P = s.P;
-  m->sched = sched ? *sched : sim_sched_from_env();
-  const SimSched& K = m->sched;
-  if (K.heavy_min != SIM_KEEP) P.heavy_min = K.heavy_min;
-  if (K.step_cap != SIM_KEEP) P.step_cap = K.step_cap;
-  if (K.sweep_epoch != SIM_KEEP) P.sweep_epoch = K.sweep_epoch;
-  if (K.sweep_blocks != SIM_KEEP) P.sweep_blocks = K.sweep_blocks;
-  if (K.pilot != SIM_KEEP) P.pilot = K.pilot;
-  if (K.force_epoch != SIM_KEEP) P.force_epoch = K.force_epoch;
-  { u32 ns = 1; for (u32 i = 0; cuts && i < cuts->n; ++i) if (cuts->kind[i] == 3) ++ns;
-    if (ns > 1) { P.pilot = 0; P.multi = ns; P.chunk_bits = K.batch_chunk_bits != SIM_KEEP ? K.batch_chunk_bits : br_batch_chunk_bits(n); } }   // (as br_job_compress_device)
-  const u32 ch = 1u << P.chunk_bits;
-  std::vector<BrBlockIn> chunks;
-  P.finish_empty = cuts && cuts->finish_empty ? 1u : 0u;
-  br_build_blocks(P, n, cuts ? cuts->pos : nullptr, cuts ? cuts->n : 0, cuts ? (cuts->is_final != 0 && !cuts->finish_empty) : true, &chunks, m->blks, nullptr, cuts ? cuts->kind : nullptr);
-  m->slot_blk.assign(((size_t)n >> P.lgblock) + 2, 0);
-  { u32 bb = 0; for (size_t i = 0; i < m->slot_blk.size(); ++i) { const u64 pp = (u64)i << P.lgblock; while (bb + 1 < m->blks.size() && m->blks[bb].end <= pp) ++bb; m->slot_blk[i] = bb; } }
-  s.slot_blk = m->slot_blk.data();
-  P.nblocks = (u32)chunks.size();
+  s.P = plan.P;
+  const BrParams& P = s.P;
+  const u32 nb = P.nblocks, words = (n + 31) / 32 + 2;
+  s.blk = plan.blk.data(); s.nblk = (u32)plan.blk.size(); s.slot_blk = plan.slot_blk.data(); s.stream_blk = plan.stream_blk.data();
   m->data.assign(in, in + n); m->data.resize(n + 64, 0);
   s.data = m->data.data();
-  u32 nb = P.nblocks, words = (n + 31) / 32 + 2;
-  m->bin = chunks; m->bin_used.resize(nb); m->bout.resize(nb);
+  m->bin_used.resize(nb); m->bout.resize(nb);
   memset(m->bin_used.data(), 0, nb * sizeof(BrBlockIn));
   memset(m->bout.data(), 0, nb * sizeof(BrBlockOut));
   m->bits_latest.assign(words, 0); m->bits_cur.assign(2 * words, 0); m->srch_latest.assign(words, 0); m->srch_cur.assign(words, 0); m->cover_cur.assign(words, 0);
-  // initial guess: everything stored except the unsearchable tail of each block
-  for (u32 k = 0; k < nb; ++k)
-    for (u32 p = m->bin[k].pos; p < m->bin[k].end && p + P.htl <= m->bin[k].blk_end; ++p) m->bits_latest[p >> 5] |= 1u << (p & 31);
-  for (size_t bi = 1; bi < m->blks.size(); ++bi) {   // StitchToPreviousBlock positions
-    const BrBlk& B = m->blks[bi];
-    if (B.end - B.start >= P.htl - 1 && B.start - B.base >= 3)
-      for (u32 q = B.start - 3; q < B.start; ++q) m->bits_latest[q >> 5] |= 1u << (q & 31);
-  }
+  s.bits_latest = m->bits_latest.data();
+  for (u32 bi = 0; bi < s.nblk; ++bi) br_init_bits(s, bi, 0, 1);   // k_init_bits
   m->storedS.assign(words + 32, 0); m->prefS.assign(n / 1024 + 4, 0);
   m->dirty.assign(nb, 0); m->changed_bits.assign(nb, 0); m->changed_epoch.assign(nb, -1); m->bitdep_epoch.assign(nb + 1, -1);
-  P.max_epochs = 4 * nb + 4096;
   m->epoch_cum.assign(P.max_epochs + 2, 0);
   m->ext_total.assign(nb, 0); m->lil_in.assign(nb, 0); m->cmd_off.assign(nb, 0); m->force_unc.assign(nb + 1, 0);
-  m->counters.assign(64, 0); m->hist.assign(256 * (size_t)(P.multi ? P.multi : 1), 0); m->mbs.resize(nb + 1);
-  if (P.multi) {
-    m->stream_blk.assign(P.multi + 1, (u32)m->blks.size());
-    for (size_t bi = m->blks.size(); bi-- > 0;) m->stream_blk[m->blks[bi].stream] = (u32)bi;
-    m->stream_nmb.assign(P.multi + 1, 0); m->stream_ncmd.assign(P.multi + 1, 0); m->mbs_stage.resize(m->blks.size());
-    s.stream_blk = m->stream_blk.data(); s.stream_nmb = m->stream_nmb.data(); s.stream_ncmd = m->stream_ncmd.data(); s.mbs_stage = m->mbs_stage.data();
-  }
-  s.cmd_stride = ch / 2 + 2;
+  m->counters.assign(64, 0); m->hist.assign(256 * (size_t)plan.nstreams, 0); m->mbs.resize(nb + 1);
+  m->stream_nmb.assign(plan.nstreams + 1, 0); m->stream_ncmd.assign(plan.nstreams + 1, 0); m->mbs_stage.resize(s.nblk);
+  s.stream_nmb = m->stream_nmb.data(); s.stream_ncmd = m->stream_ncmd.data(); s.mbs_stage = m->mbs_stage.data();
+  s.cmd_stride = plan.cmd_stride;
   m->cmd_blocks.resize((size_t)(nb + 1) * s.cmd_stride);   // (+ a guard slice behind the last chunk's: see sim_lz77_fixpoint)
-  s.bits_latest = m->bits_latest.data(); s.bits_cur = m->bits_cur.data(); s.bits_words = (u32)m->bits_latest.size();
+  s.bits_cur = m->bits_cur.data(); s.bits_words = words;
   s.srch_latest = m->srch_latest.data(); s.srch_cur = m->srch_cur.data(); s.cover_cur = m->cover_cur.data();
   s.storedS = m->storedS.data(); s.prefS = m->prefS.data();
   s.bin = m->bin.data(); s.bin_used = m->bin_used.data(); s.bout = m->bout.data();
@@ -196,24 +170,15 @@ static SimStream* sim_setup(int q, int lgwin, const u8* in, u32 n, const SimCuts
   s.ext_total = m->ext_total.data(); s.lil_in = m->lil_in.data(); s.cmd_off = m->cmd_off.data();
   s.mbs = m->mbs.data(); s.force_unc = m->force_unc.data(); s.counters = m->counters.data();
   s.hist_scratch = m->hist.data();
-  s.blk = m->blks.data(); s.nblk = (u32)m->blks.size();
-  m->blkin.resize(m->blks.size()); s.blkin = m->blkin.data();
+  m->blkin.resize(s.nblk); s.blkin = m->blkin.data();
   m->key_flips.assign(P.nbuckets + 2, 0); s.key_flips = m->key_flips.data();
   if (P.quick) { m->saw.assign(((size_t)n << P.qk_sweep_bits) + 4, 0xdeadbeefu); s.saw = m->saw.data(); }
   m->dirty_list.assign(nb + 1, 0); m->block_mb.assign(nb + 1, 0);
   s.dirty_list = m->dirty_list.data(); s.block_mb = m->block_mb.data();
-  // ran_list as the product sizes it (br_job_compress_device), followed by a guard as long again: a launch that appends
-  // more walks than the product holds writes into the guard, and the fixpoint fails the call (SIM_ERR_CAPACITY)
-  m->ran_cap = nb + 16;
-  m->ran_list.assign(2 * (size_t)m->ran_cap, 0); s.ran_list = m->ran_list.data();
-  const u8* p = g_t.blob.data() + 8;
-  s.dict_size_bits = p; p += 32;
-  s.dict_offsets = (const u32*)p; p += 128;
-  s.dict = p; p += 122784;
-  s.dict_hash_words = (const u16*)p; p += 65536;
-  s.dict_hash_lengths = p; p += 32768;
-  s.ctx_lut = p;
-  s.log2tab = g_t.log2tab.data(); s.log2tab_n = (u32)g_t.log2tab.size();
+  // ran_list followed by a guard as long again: a launch that appends more walks than the product holds writes into the
+  // guard, and the fixpoint fails the call (SIM_ERR_CAPACITY)
+  m->ran_list.assign(2 * (size_t)plan.ran_cap, 0); s.ran_list = m->ran_list.data();
+  br_bind_tables(s, g_t.blob.data(), g_t.log2tab.data(), (u32)g_t.log2tab.size());
   sim_build_sorted(*m);
   if (P.quick) {   // k_slot_pred
     m->qpred.assign(((size_t)n << P.qk_sweep_bits) + 4, 0);
@@ -274,13 +239,11 @@ static int sim_lz77_fixpoint(SimStream& m) {
     if (s.forced) ++m.st[SIM_ST_FORCED];
     { u32 nd = s.counters[5]; std::vector<u32> dl(nd); for (u32 t = 0; t < nd; ++t) dl[t] = br_sched_entry(s, t);
       for (u32 t : sim_order(nd, K.walk_order, K.walk_seed, s.epoch, 0)) { const u32 k = dl[t]; const bool f = s.forced && k == s.counters[6];
-      if (s.P.quick) { if (s.P.multi) br_walk_block<0, true>(s, k, f); else br_walk_block<0>(s, k, f); }
-      else if (s.P.multi) { if (s.P.block_bits >= 6) br_walk_block<4, true>(s, k, f); else br_walk_block<1, true>(s, k, f); }
-      else if (s.P.block_bits >= 6) br_walk_block<4>(s, k, f); else br_walk_block<1>(s, k, f); } }
+        br_walk_dispatch(s.P, [&](auto g, auto mm) { br_walk_block<decltype(g)::value, decltype(mm)::value>(s, k, f); }); } }
     m.block_runs += s.counters[4];
     if (s.counters[4] > m.st[SIM_ST_MAX_WALKS]) m.st[SIM_ST_MAX_WALKS] = s.counters[4];
-    if (s.counters[4] > m.ran_cap) {
-      fprintf(stderr, "sim: launch %u walked %u chunks, ran_list holds %u\n", s.epoch, s.counters[4], m.ran_cap);
+    if (s.counters[4] > m.plan.ran_cap) {
+      fprintf(stderr, "sim: launch %u walked %u chunks, ran_list holds %u\n", s.epoch, s.counters[4], m.plan.ran_cap);
       return SIM_ERR_CAPACITY;
     }
     for (u32 i = 0; i < s.counters[4]; ++i)
@@ -332,16 +295,14 @@ static u32 sim_verify_fixpoint(SimStream& m) {
   const std::vector<BrCmd> old_cmds(m.cmd_blocks);
   const std::vector<u32> latest0(m.bits_latest), srch0(m.srch_latest), counters0(m.counters), key_flips0(m.key_flips), saw0(m.saw), changed_bits0(m.changed_bits);
   const std::vector<int> bitdep0(m.bitdep_epoch), changed_epoch0(m.changed_epoch);
-  const std::vector<BrBlk> blks0(m.blks);
+  const std::vector<BrBlk> blks0(m.plan.blk);
   ++s.epoch;
   sim_build_storedS(m);   // (the S-ordered snapshot of the final bits: the last launch's commits are not in it yet)
   std::fill(m.bits_cur.begin(), m.bits_cur.end(), 0); std::fill(m.srch_cur.begin(), m.srch_cur.end(), 0);
   s.counters[4] = 0;
   for (u32 k = 0; k < nb; ++k) {
     BrBlockOut o; u32 sp0 = 0xffffffffu;
-    if (s.P.quick) { if (s.P.multi) br_walk_one<0, true>(s, k, s.bin[k], o, k, sp0); else br_walk_one<0>(s, k, s.bin[k], o, k, sp0); }
-    else if (s.P.multi) { if (s.P.block_bits >= 6) br_walk_one<4, true>(s, k, s.bin[k], o, k, sp0); else br_walk_one<1, true>(s, k, s.bin[k], o, k, sp0); }
-    else if (s.P.block_bits >= 6) br_walk_one<4>(s, k, s.bin[k], o, k, sp0); else br_walk_one<1>(s, k, s.bin[k], o, k, sp0);
+    br_walk_dispatch(s.P, [&](auto g, auto mm) { br_walk_one<decltype(g)::value, decltype(mm)::value>(s, k, s.bin[k], o, k, sp0); });
   }
   m.bits_prev = m.bits_latest; s.bits_prev = m.bits_prev.data();
   std::fill(m.cover_cur.begin(), m.cover_cur.end(), 0);
@@ -386,14 +347,14 @@ static u32 sim_verify_fixpoint(SimStream& m) {
   std::copy(counters0.begin(), counters0.end(), m.counters.begin()); std::copy(key_flips0.begin(), key_flips0.end(), m.key_flips.begin());
   std::copy(saw0.begin(), saw0.end(), m.saw.begin()); std::copy(changed_bits0.begin(), changed_bits0.end(), m.changed_bits.begin());
   std::copy(bitdep0.begin(), bitdep0.end(), m.bitdep_epoch.begin()); std::copy(changed_epoch0.begin(), changed_epoch0.end(), m.changed_epoch.begin());
-  std::copy(blks0.begin(), blks0.end(), m.blks.begin());
+  std::copy(blks0.begin(), blks0.end(), m.plan.blk.begin());
   return ndiff;
 }
 
 // Runs the LZ77 stage; returns the commands of every metablock back to back.
 extern "C" long sim_lz77(int q, int lgwin, const u8* in, u32 n, BrCmd* cmds_out, u32 cmds_cap,
                          u32* mb_info /* [5*i]: start,end,ncmd,compress,cmd_off */, u32 mb_cap, u32* stats) {
-  SimStream* m = sim_setup(q, lgwin, in, n);
+  SimStream* m = sim_setup(q, lgwin, n, in, n);
   if (!m) return -1;
   if (const int e = sim_lz77_fixpoint(*m)) { delete m; return e; }
   u32 nm = m->s.counters[1], total = m->s.counters[2];
@@ -411,7 +372,7 @@ extern "C" long sim_lz77(int q, int lgwin, const u8* in, u32 n, BrCmd* cmds_out,
 
 // The position index of a one-shot job as the sim builds it (the counterpart of the product's br_debug_sort hook).
 extern "C" int sim_debug_sort(int q, int lgwin, const u8* in, u32 n, u32* S_out, u32* seg_out) {
-  SimStream* m = sim_setup(q, lgwin, in, n);
+  SimStream* m = sim_setup(q, lgwin, n, in, n);
   if (!m) return 0;
   memcpy(S_out, m->S.data(), (size_t)n * 4);
   memcpy(seg_out, m->seg.data(), (size_t)(m->s.P.nbuckets + 2) * 4);
@@ -434,7 +395,7 @@ struct SimEnt {
   std::vector<u16> dist_sym;
   std::vector<BrMbAux> aux;
   std::vector<u8> scratch;
-  std::vector<u64> scratch_off, out_off;
+  BrMbLayout L;
 };
 static void sim_entropy2(SimStream& m, SimEnt& E) {
   BrStream& s = m.s;
@@ -450,34 +411,29 @@ static void sim_entropy2(SimStream& m, SimEnt& E) {
   E.lit_pos.assign(e.total_lits + 1, 0); E.lit_cmd.assign(e.total_lits + 1, 0); E.dist_sym.assign(e.total_dist + 1, 0);
   E.lit_len.assign(e.total_lits + 2, 0); E.cmd_len.assign(C + 2, 0); E.lit_bit_base.assign(C + 1, 0); E.cmd_mb.assign(C + 1, 0);
   E.aux.assign(nm, BrMbAux());
-  E.scratch_off.assign(nm, 0); E.out_off.assign(nm, 0);
-  size_t st = 0, ot = 0;
-  for (u32 i = 0; i < nm; ++i) {
-    E.scratch_off[i] = st; E.out_off[i] = ot;
-    const BrMetaBlock& mb = s.mbs[i];
-    for (u32 c = mb.cmd_off; c < mb.cmd_off + mb.ncmd; ++c) E.cmd_mb[c] = i;
-    if (mb.compress) { st += (br_mb_scratch_bytes(s.P, mb.nlit, mb.ncmd) + 255) & ~255u; ot += (2 * (size_t)(mb.end - mb.start) + 503) / 4 + 16; }
-  }
-  E.scratch.assign(st + 256, 0); E.outbits.assign(ot + 64, 0);
+  for (u32 i = 0; i < nm; ++i)
+    for (u32 c = s.mbs[i].cmd_off; c < s.mbs[i].cmd_off + s.mbs[i].ncmd; ++c) E.cmd_mb[c] = i;
+  br_mb_layout(s.P, s.mbs, nm, E.L);
+  E.scratch.assign(E.L.scratch_bytes + 256, 0); E.outbits.assign(E.L.out_words + 64, 0);
   e.lit_ord = E.lit_ord.data(); e.cmd_pos = E.cmd_pos.data(); e.dist_ord = E.dist_ord.data();
   e.lit_pos = E.lit_pos.data(); e.lit_cmd = E.lit_cmd.data(); e.dist_sym = E.dist_sym.data();
   e.lit_len = E.lit_len.data(); e.cmd_len = E.cmd_len.data(); e.lit_bit_base = E.lit_bit_base.data();
-  e.cmd_mb = E.cmd_mb.data(); e.aux = E.aux.data(); e.scratch = E.scratch.data(); e.scratch_off = E.scratch_off.data();
-  e.outbits = E.outbits.data(); e.out_off = E.out_off.data();
+  e.cmd_mb = E.cmd_mb.data(); e.aux = E.aux.data(); e.scratch = E.scratch.data(); e.scratch_off = E.L.scratch_off.data();
+  e.outbits = E.outbits.data(); e.out_off = E.L.out_off.data();
   for (u32 c = 0; c < C; c += BR_WARP) br_expand_cmds(e, c);
   std::vector<u32> smem(64 * 1024);
   for (u32 i = 0; i < nm; ++i) {
     const BrMetaBlock& mb = s.mbs[i];
     if (!mb.compress) continue;
     BrMbAux& a = E.aux[i];
-    u8* sc = E.scratch.data() + E.scratch_off[i];
+    u8* sc = E.scratch.data() + E.L.scratch_off[i];
     BrMbMem* M = (BrMbMem*)sc;
     a.which = s.P.disable_ctx ? 1u : br_decide_context_modeling(s, mb.start, mb.end - mb.start, M->sc.rle_syms);
     a.lit_base = E.lit_ord[mb.cmd_off]; a.dist_base = E.dist_ord[mb.cmd_off];
     a.nsym[0] = mb.nlit; a.nsym[1] = mb.ncmd; a.nsym[2] = E.dist_ord[mb.cmd_off + mb.ncmd] - a.dist_base;
     u32 off = br_align8((u32)sizeof(BrMbMem));
     for (int cat = 0; cat < 3; ++cat) { a.var_off[cat] = off; off += br_mb2_var_bytes(br_mb2_nblk(cat, mb.nlit, mb.ncmd)); }
-    if (s.P.mb_kind) { br_prep_flat(s, e, mb, a, sc, E.outbits.data() + E.out_off[i]); continue; }
+    if (s.P.mb_kind) { br_prep_flat(s, e, mb, a, sc, E.outbits.data() + E.L.out_off[i]); continue; }
     const u32 A[3] = {256, 704, 64}, NC[3] = {a.which, 1, 1}, MB[3] = {512, 1024, 512};
     const double TH[3] = {400.0, 500.0, 100.0};
     u32* H[3] = {M->lit_H, M->cmd_H, M->dist_H};
@@ -486,7 +442,7 @@ static void sim_entropy2(SimStream& m, SimEnt& E) {
       br_split_cta(s, e, mb, a, cat, A[cat], NC[cat], MB[cat], TH[cat], a.nsym[cat], br_mb2_types(sc, a, cat, nblk),
                    br_mb2_lengths(sc, a, cat, nblk), H[cat], smem.data());
     }
-    br_prep_codes(s, mb, a, sc, E.outbits.data() + E.out_off[i]);
+    br_prep_codes(s, mb, a, sc, E.outbits.data() + E.L.out_off[i]);
   }
   for (u32 o = 0; o < e.total_lits; ++o) br_lit_bits(s, e, o);
   for (u32 i = 0; i < C; ++i) br_cmd_bits(s, e, i);
@@ -498,13 +454,13 @@ static void sim_entropy2(SimStream& m, SimEnt& E) {
 
 // Full pipeline; returns compressed size or negative error.  cuts: see br_pipeline.h BrCuts.
 // stats: nstats words (SIM_ST_*).
-static long sim_compress_impl(int q, int lgwin, const u8* in, u32 n, u8* out, size_t out_cap, u32* stats, const SimCuts* cuts,
-                              const SimSched* sched = nullptr, u32 nstats = SIM_ST_MODEL_COST + 1) {
+static long sim_compress_impl(int q, int lgwin, u32 size_hint, const u8* in, u32 n, u8* out, size_t out_cap, u32* stats,
+                              const BrCuts* cuts, const SimSched* sched = nullptr, u32 nstats = SIM_ST_MODEL_COST + 1) {
   if (n == 0) { if (out_cap < 1) return -3; out[0] = 6; return 1; }
 #ifdef BR_SIM_DEBUG
   memset(br_sim_cnt, 0, sizeof(br_sim_cnt)); memset(br_sim_bnd, 0, sizeof(br_sim_bnd));
 #endif
-  SimStream* m = sim_setup(q, lgwin, in, n, cuts, sched);
+  SimStream* m = sim_setup(q, lgwin, size_hint, in, n, cuts, sched);
   if (!m) return -1;
   BrStream& s = m->s;
   std::vector<u8> res;
@@ -530,11 +486,11 @@ static long sim_compress_impl(int q, int lgwin, const u8* in, u32 n, u8* out, si
       for (u32 i = 0; i < nm; ++i) fprintf(stderr, "SIMMB start %u bytes %u ncmd %u nlit %u last %u compress %u bits %u\n", s.mbs[i].start, s.mbs[i].end - s.mbs[i].start,
                                            s.mbs[i].ncmd, s.mbs[i].nlit, s.mbs[i].is_last, s.mbs[i].compress, s.mbs[i].out_bits);
     // stream assembly: the shared scan (br_assemble.h), then the copies of k_assemble_copy
-    std::vector<u32> outw(((size_t)n + ((size_t)n >> 3) + 4096 + 8ull * nm) / 4 + 16, 0);
+    std::vector<u32> outw(E.L.out_cap / 4 + 16, 0);
     std::vector<BrCopyDesc> desc(nm + 1);
     std::vector<u64> cut_end((cuts ? cuts->n : 0) + 2, 0), stream_end(s.P.multi + 2, 0);
     u32 r4[4] = {0, 0, 0, 0};
-    br_assemble_scan(s, E.out_off.data(), outw.data(), desc.data(), r4, (!cuts || cuts->with_header) ? 1 : 0, cuts ? cuts->kind : nullptr,
+    br_assemble_scan(s, E.L.out_off.data(), outw.data(), desc.data(), r4, m->plan.with_header, cuts ? cuts->kind : nullptr,
                      cut_end.data(), stream_end.data());
     const bool redo = r4[2] != 0;
     if (!redo) {
@@ -554,10 +510,10 @@ static long sim_compress_impl(int q, int lgwin, const u8* in, u32 n, u8* out, si
       if (cuts && cuts->stream_end) for (u32 i = 0; i < s.P.multi; ++i) cuts->stream_end[i] = stream_end[i];
       break;
     }
-    if (rounds > 64 + (int)s.P.multi) { delete m; return -4; }
+    if (rounds > (int)m->plan.max_rounds) { delete m; return -4; }
   }
   m->st[SIM_ST_LAUNCHES] = (u32)m->iterations; m->st[SIM_ST_WALKS] = (u32)m->block_runs; m->st[SIM_ST_CHUNKS] = s.P.nblocks;
-  m->st[SIM_ST_ROUNDS] = (u32)rounds; m->st[SIM_ST_MODEL_COST] = (u32)m->model_cost; m->st[SIM_ST_RAN_CAP] = m->ran_cap;
+  m->st[SIM_ST_ROUNDS] = (u32)rounds; m->st[SIM_ST_MODEL_COST] = (u32)m->model_cost; m->st[SIM_ST_RAN_CAP] = m->plan.ran_cap;
 #ifdef BR_SIM_DEBUG
   m->st[SIM_ST_PREDICT_OK] = (u32)br_sim_bnd[0]; m->st[SIM_ST_PREDICT_NO] = (u32)br_sim_bnd[1];
 #endif
@@ -568,13 +524,13 @@ static long sim_compress_impl(int q, int lgwin, const u8* in, u32 n, u8* out, si
   return (long)res.size();
 }
 extern "C" long sim_compress(int q, int lgwin, const u8* in, u32 n, u8* out, size_t out_cap, u32* stats) {
-  return sim_compress_impl(q, lgwin, in, n, out, out_cap, stats, nullptr);
+  return sim_compress_impl(q, lgwin, n, in, n, out, out_cap, stats, nullptr);
 }
 extern "C" long sim_compress_cuts(int q, int lgwin, u32 size_hint, const u8* in, u32 n, const u32* cut_pos, const u32* cut_kind, u32 ncuts,
                                   int is_final, int with_header, int finish_empty, u64* end_bit, u8* out, size_t out_cap, u32* stats,
                                   int lgblock, int disable_ctx, u32 stream_offset) {
-  SimCuts c; c.lgblock = lgblock; c.disable_ctx = disable_ctx; c.stream_offset = stream_offset; c.pos = cut_pos; c.kind = cut_kind; c.n = ncuts; c.is_final = is_final; c.with_header = with_header; c.finish_empty = finish_empty; c.end_bit = end_bit; c.size_hint = size_hint; c.stream_end = nullptr;
-  return sim_compress_impl(q, lgwin, in, n, out, out_cap, stats, &c);
+  const BrCuts c = {cut_pos, cut_kind, ncuts, is_final, with_header, finish_empty, end_bit, lgblock, disable_ctx, stream_offset, nullptr};
+  return sim_compress_impl(q, lgwin, size_hint, in, n, out, out_cap, stats, &c);
 }
 #endif
 
@@ -634,9 +590,8 @@ static long sim_compress_multi_impl(int q, int lgwin, const u8* in, u32 n, const
   std::vector<u32> kind(nstreams, 3);
   u32 hint = 0;
   for (u32 k = 0; k < nstreams; ++k) { const u32 sz = bounds[k] - (k ? bounds[k - 1] : 0); if (sz > hint) hint = sz; }
-  SimCuts c; memset(&c, 0, sizeof(c));
-  c.pos = bounds; c.kind = kind.data(); c.n = nstreams - 1; c.is_final = 1; c.with_header = 1; c.size_hint = hint; c.stream_end = stream_end;
-  return sim_compress_impl(q, lgwin, in, n, out, out_cap, stats, &c, sched, nstats);
+  const BrCuts c = {bounds, kind.data(), nstreams - 1, 1, 1, 0, nullptr, 0, 0, 0, stream_end};
+  return sim_compress_impl(q, lgwin, hint, in, n, out, out_cap, stats, &c, sched, nstats);
 }
 extern "C" long sim_compress_multi(int q, int lgwin, const u8* in, u32 n, const u32* bounds, u32 nstreams, u64* stream_end,
                                    u8* out, size_t out_cap, u32* stats) {
@@ -655,9 +610,7 @@ extern "C" long sim_compress_sched(int q, int lgwin, const u8* in, u32 n, const 
     std::vector<u32> bounds(cut_pos, cut_pos + ncuts); bounds.push_back(n);
     return sim_compress_multi_impl(q, lgwin, in, n, bounds.data(), ncuts + 1, stream_end, out, out_cap, stats, sched, SIM_ST_WORDS);
   }
-  if (ncuts == 0) return sim_compress_impl(q, lgwin, in, n, out, out_cap, stats, nullptr, sched, SIM_ST_WORDS);
-  SimCuts c; memset(&c, 0, sizeof(c));
-  c.pos = cut_pos; c.kind = cut_kind; c.n = ncuts; c.is_final = 1; c.with_header = 1; c.size_hint = size_hint;
-  return sim_compress_impl(q, lgwin, in, n, out, out_cap, stats, &c, sched, SIM_ST_WORDS);
+  const BrCuts c = {cut_pos, cut_kind, ncuts, 1, 1, 0, nullptr, 0, 0, 0, nullptr};
+  return sim_compress_impl(q, lgwin, size_hint, in, n, out, out_cap, stats, ncuts ? &c : nullptr, sched, SIM_ST_WORDS);
 }
 #endif

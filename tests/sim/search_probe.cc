@@ -9,10 +9,8 @@ extern "C" int sim_debug_search(int quality, int lgwin, int lgblock, u32 size_hi
                                 u32* res) {
   if (n == 0 || nstreams == 0 || bounds[nstreams - 1] != n) return 0;
   std::vector<u32> kinds(nstreams, 3);
-  SimCuts c; memset(&c, 0, sizeof(c));
-  c.pos = bounds; c.kind = kinds.data(); c.n = nstreams - 1; c.is_final = 1; c.with_header = 1; c.size_hint = size_hint;
-  c.lgblock = lgblock;
-  SimStream* m = sim_setup(quality, lgwin, in, n, &c);
+  const BrCuts c = {bounds, kinds.data(), nstreams - 1, 1, 1, 0, nullptr, lgblock, 0, 0, nullptr};
+  SimStream* m = sim_setup(quality, lgwin, size_hint, in, n, &c);
   if (!m) return 0;
   BrStream& s = m->s;
   if (heavy_min) s.P.heavy_min = heavy_min;
@@ -25,9 +23,7 @@ extern "C" int sim_debug_search(int quality, int lgwin, int lgblock, u32 size_hi
   for (u32 t = 0; t < np; ++t) {
     const u32* pr = probes + (size_t)t * BR_PROBE_WORDS;
     u32* r = res + (size_t)t * BR_PROBE_WORDS;
-    if (s.P.quick) br_probe_search<0>(s, own.data(), pr, r);
-    else if (s.P.block_bits >= 6) br_probe_search<4>(s, own.data(), pr, r);
-    else br_probe_search<1>(s, own.data(), pr, r);
+    br_walk_dispatch(s.P, [&](auto g, auto) { br_probe_search<decltype(g)::value>(s, own.data(), pr, r); });
   }
   delete m;
   return 1;

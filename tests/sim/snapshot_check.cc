@@ -8,9 +8,8 @@
 // cut_pos / cut_kind / ncuts: the stream's cuts (br_pipeline.h BrCuts: kind 1 FLUSH, 3 the end of one stream of a batch).
 extern "C" int snap_check_lz77(int q, int lgwin, const u8* in, u32 n, u32 size_hint, const u32* cut_pos, const u32* cut_kind,
                                u32 ncuts, u64* stats) {
-  SimCuts c; memset(&c, 0, sizeof(c));
-  c.pos = cut_pos; c.kind = cut_kind; c.n = ncuts; c.is_final = 1; c.with_header = 1; c.size_hint = size_hint;
-  SimStream* m = sim_setup(q, lgwin, in, n, ncuts ? &c : nullptr);
+  const BrCuts c = {cut_pos, cut_kind, ncuts, 1, 1, 0, nullptr, 0, 0, 0, nullptr};
+  SimStream* m = sim_setup(q, lgwin, size_hint, in, n, ncuts ? &c : nullptr);
   if (!m) return 0;
   BrStream& s = m->s;
   if (s.P.quick) { delete m; return 0; }   // (qualities 2..4 read no snapshot)
@@ -33,8 +32,7 @@ extern "C" int snap_check_lz77(int q, int lgwin, const u8* in, u32 n, u32 size_h
     s.counters[4] = 0; s.counters[16] = 0;
     s.forced = s.epoch - round_epoch0 >= s.P.force_epoch;
     { u32 nd = s.counters[5]; std::vector<u32> dl(nd); for (u32 t = 0; t < nd; ++t) dl[t] = br_sched_entry(s, t); for (u32 k : dl) { const bool f = s.forced && k == s.counters[6];
-      if (s.P.multi) { if (s.P.block_bits >= 6) br_walk_block<4, true>(s, k, f); else br_walk_block<1, true>(s, k, f); }
-      else if (s.P.block_bits >= 6) br_walk_block<4>(s, k, f); else br_walk_block<1>(s, k, f); } }
+      br_walk_dispatch(s.P, [&](auto g, auto mm) { br_walk_block<decltype(g)::value, decltype(mm)::value>(s, k, f); }); } }
     m->bits_prev = m->bits_latest; s.bits_prev = m->bits_prev.data();
     std::fill(m->cover_cur.begin(), m->cover_cur.end(), 0);
     for (u32 i = 0; i < s.counters[4]; ++i) br_cover_run(s, s.ran_list[i]);

@@ -210,6 +210,15 @@ def test_schedule_matrix(sim, ora, name, knobs):
             check(sim, d, qq, w, sched(**knobs), _want(ora, d, qq, w), (name, label, qq, w))
 
 
+def test_sweep_blocks_not_a_power_of_two(sim):
+    """sweep_blocks must be a power of two (BrParams::sweep_blocks): the sim refuses any other value, as the product's
+    br_debug_compress_sched does"""
+    d = _noise(20000, 11)
+    for b in (0, 3, 24):
+        r, _, _ = run(sim, d, 5, 22, sched(sweep_blocks=b))
+        assert r < 0, b
+
+
 def test_jacobi_only(sim, ora):
     """sweep_epoch beyond any launch: no sweep ever, every dirty chunk walked on its own until the fixpoint (the forced
     walker still ends it)"""
