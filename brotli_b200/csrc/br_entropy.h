@@ -14,7 +14,7 @@
 
 // ------------------------------------------------------------------ bit writer
 // per_thread = 0: the cursor is warp-uniform and lane 0 writes; 1: the writer belongs to ONE thread (parallel tree
-// storing in br_prep_codes).  out = nullptr: count bits only.
+// storing in br_code_build / br_code_store).  out = nullptr: count bits only.
 struct BrBitW { u32* out; u32 ix; u32 per_thread; };
 // LSB-first append (write_bits.h:33).  The buffer is pre-zeroed and every write is an atomic
 // OR (RED at L2), so lane-0 serial writes and lane-parallel writes can interleave freely.

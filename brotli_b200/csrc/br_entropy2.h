@@ -10,8 +10,9 @@
 //                                       metablock_inc.h:86 is serial, but each link is executed by a
 //                                       whole CTA (histogram accumulation with shared-memory atomics,
 //                                       the 3 x contexts entropy sums on separate threads)
-//   E4  br_prep_codes                   smoothing + Huffman construction of every histogram in
-//                                       parallel, then header / trees stored by one thread
+//   E4  br_code_build / br_mb_header    smoothing + Huffman construction of every prefix code of the job
+//       / br_code_store                 in parallel, the header by one warp per metablock, then every
+//                                       code stored at its offset in parallel
 //   E5  br_lit_bits / br_cmd_bits       per-symbol bit counts; prefix sums give every symbol its
 //                                       absolute bit offset (the north-star "prefix-sum packing")
 //   E6  br_emit_lit / br_emit_cmd       scatter of the code words with atomic OR
@@ -44,12 +45,35 @@ struct BrMbAux {
 struct BrBlockInfo { u32 start; u32 sw_nbits; u64 sw_bits; u32 type; u32 pad; };
 
 BR_HD u32 br_mb2_var_bytes(u32 nblk) { return br_align8(nblk * ((u32)sizeof(BrBlockInfo) + 4) + nblk) + 8; }
-#define BR_PREP_THREADS 64
+#define BR_CODE_BITS_WORDS (3 * 256 + 8)
 BR_HD u32 br_mb2_scratch_bytes(u32 nlit, u32 ncmd) {
   u32 lb = nlit / 512 + 2, cb = ncmd / 1024 + 2, db = ncmd / 512 + 2;
   return br_align8((u32)sizeof(BrMbMem)) + br_mb2_var_bytes(lb) + br_mb2_var_bytes(cb) + br_mb2_var_bytes(db) +
-         BR_PREP_THREADS * (u32)sizeof(BrHTree) * (2 * 704 + 2) + (3 * 256 + 8) * 4;   // + sizes / offsets of the stored codes
+         BR_CODE_BITS_WORDS * 4;   // + sizes / offsets of the stored codes
 }
+// [nl + ncm + nd + 1]: the stored size of every prefix code of the metablock, then (br_mb_header) its bit offset
+BR_DEV u32* br_mb2_code_bits(u8* scratch, const BrMetaBlock& mb) {
+  return (u32*)(scratch + br_mb2_scratch_bytes(mb.nlit, mb.ncmd) - BR_CODE_BITS_WORDS * 4);
+}
+// Most prefix codes a metablock can have: a literal code per (block type, context) and a command and a distance code per
+// block type.  A split has at most one type per block and at most 256 / contexts types (up to 13 contexts).
+BR_HD u32 br_mb2_code_bound(u32 nlit, u32 ncmd) {
+  const u32 lb = nlit / 512 + 2, cb = ncmd / 1024 + 2, db = ncmd / 512 + 2;
+  return (13 * lb < 256 ? 13 * lb : 256) + (cb < 256 ? cb : 256) + (db < 256 ? db : 256);
+}
+// Prefix codes of a job (E4) are built and stored either by a warp each, on a copy in shared memory (BrCodeSmem), when
+// the job has at most BR_CODE_WARP_MAX of them, or else by a thread each.  A thread worker's tree area (the Huffman tree
+// of the largest alphabet, which the store reuses as its BrTreeSc) comes from a pool of the job: BR_CODE_TREE_NODES each,
+// for at most BR_CODE_THREADS_MAX workers.
+#define BR_CODE_TREE_NODES (2 * 704 + 2)
+#define BR_CODE_WARP_MAX 8192u
+#define BR_CODE_THREADS_MAX 65536u
+struct BrCodeSmem {
+  BrHTree tree[BR_CODE_TREE_NODES];
+  u32 H[704];
+  u16 bits[704];
+  u8 depth[704], good[704];
+};
 BR_DEV BrBlockInfo* br_mb2_blocks(u8* scratch, const BrMbAux& a, int cat) { return (BrBlockInfo*)(scratch + a.var_off[cat]); }
 BR_DEV u32* br_mb2_lengths(u8* scratch, const BrMbAux& a, int cat, u32 nblk) {
   return (u32*)(scratch + a.var_off[cat] + nblk * (u32)sizeof(BrBlockInfo));
@@ -271,58 +295,46 @@ BR_DEV void br_split_cta(const BrStream& st, const BrEnt& e, const BrMetaBlock& 
 }
 
 // ---------------------------------------------------------------------------------- E4
-// CTA per metablock: codes of all histograms in parallel, then warp 0 writes the metablock
-// header (brotli_bit_stream.c:947-1060) and the block tables used by E5/E6.
-BR_DEV void br_prep_codes(const BrStream& st, const BrMetaBlock& mb, BrMbAux& a, u8* scratch, u32* out) {
-  const u32 tid = BR_CTA_TID, nt = BR_CTA_N;
+// Three job-wide phases (brotli_bit_stream.c:947-1060 and :349 BuildAndStoreHuffmanTree).  Every prefix code of the job
+// is built by one worker, which also measures how many bits its serialised form takes (the store, run against a counting
+// writer).  Then one warp per metablock writes the header in front of the codes, turns the code sizes into bit offsets
+// and fills the block tables used by E5/E6.  Then the workers store their codes at those offsets: all writes are atomic
+// ORs.  A code's global index t maps to (metablock, code) through code_base, the exclusive scan of br_mb_code_count.
+BR_DEV u32 br_mb_code_count(const BrMbAux& a) { return a.num_types[0] * a.which + a.num_types[1] + a.num_types[2]; }
+// code x of a metablock: literal codes (type * contexts + context), then command codes, then distance codes
+BR_DEV u32 br_code_ref(BrMbMem* M, const BrMbAux& a, u32 x, u32** H, u8** dep, u16** bits) {
+  const u32 nl = a.num_types[0] * a.which, ncm = a.num_types[1];
+  if (x < nl) { *H = M->lit_H + x * 256; *dep = M->lit_depth + x * 256; *bits = M->lit_bits + x * 256; return 256; }
+  if (x < nl + ncm) { x -= nl; *H = M->cmd_H + x * 704; *dep = M->cmd_depth + x * 704; *bits = M->cmd_bits + x * 704; return 704; }
+  x -= nl + ncm;
+  *H = M->dist_H + x * 64; *dep = M->dist_depth + x * 64; *bits = M->dist_bits + x * 64; return 64;
+}
+// Smoothing, Huffman construction and the counting store of code x; tree: BR_CODE_TREE_NODES of the worker's own.
+BR_DEV void br_code_build(const BrMetaBlock& mb, const BrMbAux& a, u8* scratch, u32 x, BrHTree* tree) {
   BrMbMem* M = (BrMbMem*)scratch;
+  u32* H; u8* dep; u16* bits;
+  const u32 len = br_code_ref(M, a, x, &H, &dep, &bits);
+  u8 good[704];
+  br_optimize_counts_for_rle(len, H, good);
+  br_build_tree(H, len, tree, dep, bits);
+  BrBitW cw; cw.out = nullptr; cw.ix = 0; cw.per_thread = 1;
+  br_store_tree(H, len, len, (BrTreeSc*)tree, dep, cw);   // (the big tree is done: its memory is the store's scratch)
+  br_mb2_code_bits(scratch, mb)[x] = cw.ix;
+}
+// One warp: MapStaticContexts, the metablock header up to the codes, the code offsets and the block tables.
+BR_DEV void br_mb_header(const BrStream& st, const BrMetaBlock& mb, BrMbAux& a, u8* scratch, u32* out) {
+  BrMbMem* M = (BrMbMem*)scratch;
+  const int lane = br_lane();
   const u32 nctx = a.which;
-  const u32 nl = a.num_types[0] * nctx, ncm = a.num_types[1], nd = a.num_types[2];
-  BrHTree* trees = (BrHTree*)(scratch + br_mb2_scratch_bytes(mb.nlit, mb.ncmd) - BR_PREP_THREADS * (u32)sizeof(BrHTree) * (2 * 704 + 2) - (3 * 256 + 8) * 4);
-  BrHTree* mytree = trees + (size_t)(tid % BR_PREP_THREADS) * (2 * 704 + 2);
-  // Every prefix code of the metablock is built by its own thread, which also measures how many bits its serialised form
-  // takes (brotli_bit_stream.c:349: the store, run against a counting writer).  Once the header in front of the codes is
-  // written the offsets are known and the same threads store their codes in parallel: all writes are atomic ORs.
-  u32* tree_bits = (u32*)(trees + (size_t)BR_PREP_THREADS * (2 * 704 + 2));   // [nl + ncm + nd] sizes, then bit offsets
-  const u32 ntrees = nl + ncm + nd;
-  const u32 stride = nt < BR_PREP_THREADS ? nt : BR_PREP_THREADS;
-  if (tid < BR_PREP_THREADS) {
-    for (u32 t = tid; t < ntrees; t += stride) {
-      u8 good[704];
-      const u32* H; u8* dep; u32 len;
-      if (t < nl) {
-        H = M->lit_H + t * 256; dep = M->lit_depth + t * 256; len = 256;
-        br_optimize_counts_for_rle(256, M->lit_H + t * 256, good);
-        br_build_tree(H, 256, mytree, dep, M->lit_bits + t * 256);
-      } else if (t < nl + ncm) {
-        u32 x = t - nl;
-        H = M->cmd_H + x * 704; dep = M->cmd_depth + x * 704; len = 704;
-        br_optimize_counts_for_rle(704, M->cmd_H + x * 704, good);
-        br_build_tree(H, 704, mytree, dep, M->cmd_bits + x * 704);
-      } else {
-        u32 x = t - nl - ncm;
-        H = M->dist_H + x * 64; dep = M->dist_depth + x * 64; len = 64;
-        br_optimize_counts_for_rle(64, M->dist_H + x * 64, good);
-        br_build_tree(H, 64, mytree, dep, M->dist_bits + x * 64);
-      }
-      BrBitW cw; cw.out = nullptr; cw.ix = 0; cw.per_thread = 1;
-      br_store_tree(H, len, len, (BrTreeSc*)mytree, dep, cw);   // (the big tree is done: its memory is the store's scratch)
-      tree_bits[t] = cw.ix;
-    }
-  }
+  const u32 nl = a.num_types[0] * nctx, nd = a.num_types[2], ntrees = br_mb_code_count(a);
+  u32* code_bits = br_mb2_code_bits(scratch, mb);
   // metablock.c:677 MapStaticContexts
   if (nctx > 1)
-    for (u32 x = tid; x < (a.num_types[0] << 6); x += nt) M->cmap[x] = (x >> 6) * nctx + br_static_ctx_map((int)nctx, x & 63);
-#if BR_GPU
-  __threadfence_block();
-#endif
-  br_cta_sync();
-  const int lane = br_lane();
+    for (u32 x = (u32)lane; x < (a.num_types[0] << 6); x += BR_WARP) M->cmap[x] = (x >> 6) * nctx + br_static_ctx_map((int)nctx, x & 63);
+  br_syncwarp();
   BrMbScratch* sc = &M->sc;
   const u32 cmap_size = nctx > 1 ? (a.num_types[0] << 6) : 0;
   BrBitW w; w.out = out; w.ix = 0; w.per_thread = 0;
-  if (tid < BR_WARP) {
-  // ---- warp 0: header in front of the codes, warp-uniform
   br_put_bits(w, 1, (u64)mb.is_last);
   if (mb.is_last) br_put_bits(w, 1, 0);
   br_store_mlen(mb.end - mb.start, w);
@@ -342,26 +354,17 @@ BR_DEV void br_prep_codes(const BrStream& st, const BrMetaBlock& mb, BrMbAux& a,
   if (cmap_size == 0) br_store_trivial_context_map(nl, 6, sc, w);
   else br_encode_context_map(M->cmap, cmap_size, nl, sc, w);
   br_store_trivial_context_map(nd, 2, sc, w);
-  if (lane == 0) {   // sizes -> bit offsets
-    u32 acc = w.ix;
-    for (u32 t = 0; t < ntrees; ++t) { const u32 v = tree_bits[t]; tree_bits[t] = acc; acc += v; }
-    tree_bits[ntrees] = acc;
+  // code sizes -> bit offsets: a warp-wide exclusive scan, 32 codes at a time
+  u32 acc = w.ix;
+  for (u32 t0 = 0; t0 < ntrees; t0 += BR_WARP) {
+    const u32 t = t0 + (u32)lane;
+    u32 total;
+    const u32 ex = br_warp_excl_scan(t < ntrees ? code_bits[t] : 0u, &total);
+    if (t < ntrees) code_bits[t] = acc + ex;
+    acc += total;
   }
-  }
-#if BR_GPU
-  __threadfence_block();
-#endif
-  br_cta_sync();
-  if (tid < BR_PREP_THREADS) {
-    for (u32 t = tid; t < ntrees; t += stride) {
-      BrBitW tw; tw.out = out; tw.ix = tree_bits[t]; tw.per_thread = 1;
-      if (t < nl) br_store_tree(M->lit_H + t * 256, 256, 256, (BrTreeSc*)mytree, M->lit_depth + t * 256, tw);
-      else if (t < nl + ncm) { const u32 x = t - nl; br_store_tree(M->cmd_H + x * 704, 704, 704, (BrTreeSc*)mytree, M->cmd_depth + x * 704, tw); }
-      else { const u32 x = t - nl - ncm; br_store_tree(M->dist_H + x * 64, 64, 64, (BrTreeSc*)mytree, M->dist_depth + x * 64, tw); }
-    }
-  }
-  if (tid >= BR_WARP) return;
-  w.ix = tree_bits[ntrees];
+  if (lane == 0) code_bits[ntrees] = acc;
+  w.ix = acc;
   // ---- block tables: start ordinal of every block and the block-switch bits that precede it
   for (int cat = 0; cat < 3; ++cat) {
     u32 nblk = br_mb2_nblk(cat, mb.nlit, mb.ncmd);
@@ -390,6 +393,125 @@ BR_DEV void br_prep_codes(const BrStream& st, const BrMetaBlock& mb, BrMbAux& a,
   br_syncwarp();
   if (lane == 0) { a.hdr_bits = w.ix; a.cmap_size = cmap_size; }
 }
+// Code x stored at the offset br_mb_header gave it.
+BR_DEV void br_code_store(const BrMetaBlock& mb, const BrMbAux& a, u8* scratch, u32 x, BrHTree* tree, u32* out) {
+  BrMbMem* M = (BrMbMem*)scratch;
+  u32* H; u8* dep; u16* bits;
+  const u32 len = br_code_ref(M, a, x, &H, &dep, &bits);
+  BrBitW tw; tw.out = out; tw.ix = br_mb2_code_bits(scratch, mb)[x]; tw.per_thread = 1;
+  br_store_tree(H, len, len, (BrTreeSc*)tree, dep, tw);
+}
+
+// ---- the same two steps by one warp, on a copy of the code in shared memory
+// entropy_encode.c:68 BrotliCreateHuffmanTree with the sort spread over the lanes: every node's place is the number of
+// nodes before it in the order of br_htree_less, a strict total order on (count, symbol), so this is the permutation the
+// serial sort gives.  The merge and BrotliSetDepth run on lane 0.
+BR_DEV u64 br_htree_key(const BrHTree& t) { return ((u64)t.count << 16) | (u32)(0xFFFF - t.right_or_value); }
+BR_DEV void br_create_huffman_tree_warp(const u32* data, u32 length, int tree_limit, BrHTree* tree, u8* depth) {
+  const int lane = br_lane();
+  BrHTree* src = tree + 704;   // the unsorted nodes (n <= 704: tree[0, n) and src[0, n) are apart)
+  for (u32 count_limit = 1;; count_limit *= 2) {
+    u32 n = 0;
+    for (u32 base = 0; base < length; base += BR_WARP) {   // nonzero symbols, from the last down
+      const u32 k = base + (u32)lane, i = length - 1 - k;
+      const u32 v = k < length ? data[i] : 0u;
+      const u32 m = br_ballot(v != 0);
+      if (v) {
+        BrHTree t; t.count = v > count_limit ? v : count_limit; t.left = -1; t.right_or_value = (short)i;
+        src[n + (u32)br_popc(m & br_lanemask_lt())] = t;
+      }
+      n += (u32)br_popc(m);
+    }
+    br_syncwarp();
+    if (n == 1) { if (lane == 0) depth[src[0].right_or_value] = 1; br_syncwarp(); break; }
+    for (u32 g0 = 0; g0 < n; g0 += 8 * BR_WARP) {
+      u64 key[8]; u32 rk[8];
+      for (int r = 0; r < 8; ++r) {
+        const u32 ix = g0 + (u32)r * BR_WARP + (u32)lane;
+        key[r] = ix < n ? br_htree_key(src[ix]) : ~0ull; rk[r] = 0;
+      }
+      for (u32 j = 0; j < n; ++j) {
+        const u64 kj = br_htree_key(src[j]);
+        for (int r = 0; r < 8; ++r) rk[r] += kj < key[r] ? 1u : 0u;
+      }
+      for (int r = 0; r < 8; ++r) {
+        const u32 ix = g0 + (u32)r * BR_WARP + (u32)lane;
+        if (ix < n) tree[rk[r]] = src[ix];
+      }
+    }
+    br_syncwarp();
+    int ok = 0;
+    if (lane == 0) {
+      BrHTree sentinel; sentinel.count = 0xFFFFFFFFu; sentinel.left = -1; sentinel.right_or_value = -1;
+      tree[n] = sentinel; tree[n + 1] = sentinel;
+      u32 i = 0, j = n + 1;
+      for (u32 k = n - 1; k != 0; --k) {
+        u32 left, right;
+        if (tree[i].count <= tree[j].count) { left = i; ++i; } else { left = j; ++j; }
+        if (tree[i].count <= tree[j].count) { right = i; ++i; } else { right = j; ++j; }
+        u32 j_end = 2 * n - k;
+        tree[j_end].count = tree[left].count + tree[right].count;
+        tree[j_end].left = (short)left;
+        tree[j_end].right_or_value = (short)right;
+        tree[j_end + 1] = sentinel;
+      }
+      ok = br_set_depth((int)(2 * n - 1), tree, depth, tree_limit);
+    }
+    ok = br_shfl(ok, 0);
+    br_syncwarp();
+    if (ok) break;
+  }
+}
+// br_code_build by one warp.  S->depth and S->bits start zeroed.
+BR_DEV void br_code_build_warp(const BrMetaBlock& mb, const BrMbAux& a, u8* scratch, u32 x, BrCodeSmem* S) {
+  BrMbMem* M = (BrMbMem*)scratch;
+  const int lane = br_lane();
+  u32* H; u8* dep; u16* bits;
+  const u32 len = br_code_ref(M, a, x, &H, &dep, &bits);
+  for (u32 i = (u32)lane; i < len; i += BR_WARP) { S->H[i] = H[i]; S->depth[i] = 0; S->bits[i] = 0; }
+  br_syncwarp();
+  if (lane == 0) br_optimize_counts_for_rle(len, S->H, S->good);
+  br_syncwarp();
+  u32 count = 0;   // br_build_tree: a code of one symbol (or none) keeps depth 0
+  for (u32 base = 0; base < len && count <= 1; base += BR_WARP) count += (u32)br_popc(br_ballot(base + (u32)lane < len && S->H[base + lane]));
+  if (count > 1) {
+    br_create_huffman_tree_warp(S->H, len, 15, S->tree, S->depth);
+    if (lane == 0) br_depths_to_symbols(S->depth, len, S->bits);
+    br_syncwarp();
+  }
+  if (lane == 0) {
+    BrBitW cw; cw.out = nullptr; cw.ix = 0; cw.per_thread = 1;
+    br_store_tree(S->H, len, len, (BrTreeSc*)S->tree, S->depth, cw);
+    br_mb2_code_bits(scratch, mb)[x] = cw.ix;
+  }
+  for (u32 i = (u32)lane; i < len; i += BR_WARP) { H[i] = S->H[i]; dep[i] = S->depth[i]; bits[i] = S->bits[i]; }
+  br_syncwarp();
+}
+// br_code_store by one warp (lane 0 writes, from the shared copy)
+BR_DEV void br_code_store_warp(const BrMetaBlock& mb, const BrMbAux& a, u8* scratch, u32 x, BrCodeSmem* S, u32* out) {
+  BrMbMem* M = (BrMbMem*)scratch;
+  const int lane = br_lane();
+  u32* H; u8* dep; u16* bits;
+  const u32 len = br_code_ref(M, a, x, &H, &dep, &bits);
+  for (u32 i = (u32)lane; i < len; i += BR_WARP) { S->H[i] = H[i]; S->depth[i] = dep[i]; }
+  br_syncwarp();
+  if (lane == 0) {
+    BrBitW tw; tw.out = out; tw.ix = br_mb2_code_bits(scratch, mb)[x]; tw.per_thread = 1;
+    br_store_tree(S->H, len, len, (BrTreeSc*)S->tree, S->depth, tw);
+  }
+  br_syncwarp();
+}
+#if !BR_GPU
+// E4 of one metablock, for the CPU simulation (tests/sim), which runs the entropy stage metablock by metablock: every
+// code built, the header, every code stored, by the warp workers' functions.  The job-wide phase order of the device
+// gives the same bytes: each phase of a metablock reads and writes only that metablock's scratch and bit buffer.
+BR_DEV void br_prep_codes(const BrStream& st, const BrMetaBlock& mb, BrMbAux& a, u8* scratch, u32* out) {
+  BrCodeSmem S;
+  for (u32 x = 0; x < br_mb_code_count(a); ++x) br_code_build_warp(mb, a, scratch, x, &S);
+  br_mb_header(st, mb, a, scratch, out);
+  for (u32 x = 0; x < br_mb_code_count(a); ++x) br_code_store_warp(mb, a, scratch, x, &S, out);
+}
+#endif
 
 // ---------------------------------------------------------------------------------- E5 / E6
 BR_DEV u32 br_block_of(const BrBlockInfo* bi, u32 nb, u32 o) {
@@ -520,16 +642,23 @@ BR_DEV void br_emit_lit(const BrStream& st, const BrEnt& e, u32 o) {
 struct BrMbLayout {
   std::vector<u64> scratch_off, out_off;
   size_t scratch_bytes, out_words, out_cap;
+  u32 code_warps;     // warp workers for the prefix codes of the job (E4): one per code, when there are few enough
+  u32 code_workers;   // thread workers for the prefix codes of the job (E4), each with BR_CODE_TREE_NODES of tree area
 };
 static inline void br_mb_layout(const BrParams& P, const BrMetaBlock* mbs, u32 n_mbs, BrMbLayout& L) {
   L.scratch_off.assign(n_mbs, 0); L.out_off.assign(n_mbs, 0);
   L.scratch_bytes = L.out_words = 0;
+  u64 codes = 0;
   for (u32 i = 0; i < n_mbs; ++i) {
     L.scratch_off[i] = L.scratch_bytes; L.out_off[i] = L.out_words;
     if (mbs[i].compress) {
       L.scratch_bytes += ((size_t)br_mb_scratch_bytes(P, mbs[i].nlit, mbs[i].ncmd) + 255) & ~(size_t)255;
       L.out_words += (2 * (size_t)(mbs[i].end - mbs[i].start) + 503) / 4 + 16;
+      codes += br_mb2_code_bound(mbs[i].nlit, mbs[i].ncmd);
     }
   }
+  // (a job that may have no more codes than the warps take never needs the thread workers)
+  L.code_warps = P.mb_kind ? 0u : (u32)(codes < BR_CODE_WARP_MAX ? codes : BR_CODE_WARP_MAX);
+  L.code_workers = P.mb_kind || codes <= BR_CODE_WARP_MAX ? 0u : (u32)(codes < BR_CODE_THREADS_MAX ? codes : BR_CODE_THREADS_MAX);
   L.out_cap = (size_t)P.n + ((size_t)P.n >> 3) + 4096 + 8ull * n_mbs;
 }

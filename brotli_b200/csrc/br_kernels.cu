@@ -398,11 +398,44 @@ __global__ void __launch_bounds__(256) k_split(BrStream s, BrEnt e) {
   br_split_cta(s, e, mb, a, cat, A, nc, minb, thr, a.nsym[cat], br_mb2_types(sc, a, cat, nblk),
                br_mb2_lengths(sc, a, cat, nblk), H, sm);
 }
-__global__ void __launch_bounds__(64) k_prep(BrStream s, BrEnt e) {
+// E4 (br_entropy2.h): code_base[i] = number of prefix codes of metablock i (0 when it is stored raw), then scanned
+__global__ void k_code_count(BrStream s, BrEnt e, u32* code_base, u32 n_mbs) {
+  const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_mbs) code_base[i] = s.mbs[i].compress ? br_mb_code_count(e.aux[i]) : 0u;
+  else if (i == n_mbs) code_base[i] = 0;
+}
+// At most BR_CODE_WARP_MAX codes in the job: one warp per code, (metablock, code) of global code t from the scanned counts.
+template <bool STORE>
+__global__ void __launch_bounds__(32) k_codes_warp(BrStream s, BrEnt e, const u32* __restrict__ code_base, u32 n_mbs) {
+  __shared__ BrCodeSmem S;
+  const u32 total = code_base[n_mbs], t = blockIdx.x;
+  if (total > BR_CODE_WARP_MAX || t >= total) return;
+  const u32 m = br_upper_index(code_base, n_mbs, t);
+  const BrMetaBlock& mb = s.mbs[m];
+  u8* sc = e.scratch + e.scratch_off[m];
+  if (STORE) br_code_store_warp(mb, e.aux[m], sc, t - code_base[m], &S, e.outbits + e.out_off[m]);
+  else br_code_build_warp(mb, e.aux[m], sc, t - code_base[m], &S);
+}
+// More codes: one thread per code, every worker taking the codes gridDim.x * blockDim.x apart.
+template <bool STORE>
+__global__ void __launch_bounds__(64) k_codes(BrStream s, BrEnt e, const u32* __restrict__ code_base, u32 n_mbs, BrHTree* pool) {
+  const u32 wk = blockIdx.x * blockDim.x + threadIdx.x, nwk = gridDim.x * blockDim.x;
+  BrHTree* tree = pool + (size_t)wk * BR_CODE_TREE_NODES;
+  const u32 total = code_base[n_mbs];
+  if (total <= BR_CODE_WARP_MAX) return;
+  for (u32 t = wk; t < total; t += nwk) {
+    const u32 m = br_upper_index(code_base, n_mbs, t);
+    const BrMetaBlock& mb = s.mbs[m];
+    u8* sc = e.scratch + e.scratch_off[m];
+    if (STORE) br_code_store(mb, e.aux[m], sc, t - code_base[m], tree, e.outbits + e.out_off[m]);
+    else br_code_build(mb, e.aux[m], sc, t - code_base[m], tree);
+  }
+}
+__global__ void __launch_bounds__(32) k_mb_header(BrStream s, BrEnt e) {
   const u32 i = blockIdx.x;
   const BrMetaBlock mb = s.mbs[i];
   if (!mb.compress) return;
-  br_prep_codes(s, mb, e.aux[i], e.scratch + e.scratch_off[i], e.outbits + e.out_off[i]);
+  br_mb_header(s, mb, e.aux[i], e.scratch + e.scratch_off[i], e.outbits + e.out_off[i]);
 }
 // qualities 2, 3: histograms + the three codes of a metablock without block splits (br_entropy_flat.h)
 __global__ void __launch_bounds__(64) k_prep_flat(BrStream s, BrEnt e) {
@@ -770,7 +803,8 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
     br_mb_layout(P, hm.data(), n_mbs, L);
     const size_t C = total_cmds;
     BrEnt e; memset(&e, 0, sizeof(e));
-    BrCmd* cmds_all; u64 *soff, *ooff; BrCopyDesc* desc; u32 *out, *res, *lit_ord, *cmd_pos, *dist_ord, *stmp;
+    BrCmd* cmds_all; u64 *soff, *ooff; BrCopyDesc* desc; u32 *out, *res, *lit_ord, *cmd_pos, *dist_ord, *stmp, *code_base;
+    BrHTree* tree_pool;
     auto carve2 = [&](BrCarve& B) {
       e.scratch = B.take<u8>(L.scratch_bytes + 256); e.outbits = B.take<u32>(L.out_words + 64);
       out = B.take<u32>(L.out_cap / 4 + 16); e.cmds = cmds_all = B.take<BrCmd>(C + 1);
@@ -781,6 +815,8 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
       e.dist_sym = B.take<u16>(C + 2);
       e.lit_pos = B.take<u32>((size_t)n + 2); e.lit_cmd = B.take<u32>((size_t)n + 2); e.lit_len = B.take<u32>((size_t)n + 2);
       e.aux = B.take<BrMbAux>(n_mbs);
+      code_base = B.take<u32>(n_mbs + 1);
+      tree_pool = B.take<BrHTree>((size_t)((L.code_workers + 63) & ~63u) * BR_CODE_TREE_NODES);
       stmp = B.take<u32>(scan_tmp_words((size_t)n + C + 8) * 2);
     };
     if (!br_carve(job->arena2, carve2)) return 0;
@@ -809,7 +845,15 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
       const size_t smem_split = br_split_smem_bytes(256, 13) > br_split_smem_bytes(704, 1) ? br_split_smem_bytes(256, 13) : br_split_smem_bytes(704, 1);
       CK(cudaFuncSetAttribute(k_split, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_split));
       k_split<<<dim3(n_mbs, 3), 256, smem_split, st>>>(s, e);
-      k_prep<<<n_mbs, 64, 0, st>>>(s, e);
+      // E4: every prefix code of the job built by its own worker, the headers, then every code stored
+      k_code_count<<<(n_mbs + 1 + 255) / 256, 256, 0, st>>>(s, e, code_base, n_mbs);
+      scan_exclusive(code_base, n_mbs + 1, stmp, st);
+      const u32 code_ctas = (L.code_workers + 63) / 64;
+      if (L.code_warps) k_codes_warp<false><<<L.code_warps, 32, 0, st>>>(s, e, code_base, n_mbs);
+      if (code_ctas) k_codes<false><<<code_ctas, 64, 0, st>>>(s, e, code_base, n_mbs, tree_pool);
+      k_mb_header<<<n_mbs, 32, 0, st>>>(s, e);
+      if (L.code_warps) k_codes_warp<true><<<L.code_warps, 32, 0, st>>>(s, e, code_base, n_mbs);
+      if (code_ctas) k_codes<true><<<code_ctas, 64, 0, st>>>(s, e, code_base, n_mbs, tree_pool);
     }
     k_lit_bits<<<(e.total_lits + 1 + 255) / 256, 256, 0, st>>>(s, e);
     k_cmd_bits<<<(u32)((C + 1 + 255) / 256), 256, 0, st>>>(s, e);
@@ -819,7 +863,7 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
     if (e.total_lits) k_emit_lit<<<(e.total_lits + 255) / 256, 256, 0, st>>>(s, e);
     cudaEventRecord(ev[9], st);
     cudaEventRecord(ev[3], st);
-    ++job->stats.encode_launches; job->stats.launches += 24;
+    ++job->stats.encode_launches; job->stats.launches += 28;
     k_assemble_scan<<<1, 32, 0, st>>>(s, ooff, out, desc, res, plan.with_header, cut_kind, cut_end, stream_end);
     CK(cudaMemcpyAsync(hp + 16, res, 16, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));

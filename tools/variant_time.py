@@ -4,8 +4,8 @@ usage: variant_time.py [--inputs text5,web5,text6,bin9] [--rounds R] LIB.so [LIB
   LIB.so: a build of libbrotlienc_b200.so (a path, or a name under brotli_b200/).
   Every round runs each library once per input, in turn, after one untimed warm-up call per library and input, so
   that clock and thermal drift fall on every build alike.  Prints, per input and library, the median and the min-max
-  of ms_walk, ms_index, ms_lz77 - ms_walk (the LZ77 stage outside the walker: chain, commits, snapshot upkeep) and
-  ms_total (the library's own stage timers, CUDA events) and whether every build returned the same bytes.
+  of ms_walk, ms_index, ms_lz77 - ms_walk (the LZ77 stage outside the walker: chain, commits, snapshot upkeep),
+  ms_entropy and ms_total (the library's own stage timers, CUDA events) and whether every build returned the same bytes.
 inputs:
   text5  100 MB synthetic text (the headline's synth_text, seed 20250922), quality 5, lgwin 22
   web5   256 MiB of the synthetic web mix (synth_web, seed 20250923: the web config's generator), quality 5, lgwin 22
@@ -58,14 +58,14 @@ for name in a.inputs.split(","):
             out, st = run(so, d, q, w)
             if out != outs[so]:
                 outs[so] = None
-            res[so].append((st["ms_walk"], st["ms_index"], st["ms_lz77"] - st["ms_walk"], st["ms_total"]))
+            res[so].append((st["ms_walk"], st["ms_index"], st["ms_lz77"] - st["ms_walk"], st["ms_entropy"], st["ms_total"]))
     same = len({o for o in outs.values()}) == 1 and None not in outs.values()
     print("%s: %d bytes, quality %d, lgwin %d, %d rounds; outputs identical across builds and rounds: %s" % (
         name, len(d), q, w, a.rounds, same), flush=True)
     for so in a.libs:
         cols = []
-        for i, label in enumerate(("walk", "index", "lz77-walk", "total")):
+        for i, label in enumerate(("walk", "index", "lz77-walk", "entropy", "total")):
             v = [r[i] for r in res[so]]
             cols.append("%s median %7.2f ms (%.2f-%.2f)" % (label, statistics.median(v), min(v), max(v)))
-        print("  %-40s %s  MB/s %.0f" % (so, "  ".join(cols), len(d) / 1e3 / statistics.median([r[3] for r in res[so]])),
+        print("  %-40s %s  MB/s %.0f" % (so, "  ".join(cols), len(d) / 1e3 / statistics.median([r[4] for r in res[so]])),
               flush=True)
