@@ -662,3 +662,76 @@ static inline void br_mb_layout(const BrParams& P, const BrMetaBlock* mbs, u32 n
   L.code_workers = P.mb_kind || codes <= BR_CODE_WARP_MAX ? 0u : (u32)(codes < BR_CODE_THREADS_MAX ? codes : BR_CODE_THREADS_MAX);
   L.out_cap = (size_t)P.n + ((size_t)P.n >> 3) + 4096 + 8ull * n_mbs;
 }
+
+// Host: n synthetic metablocks for E4 alone (the test hooks br_debug_codes and tests/sim sim_debug_codes).  counts[3 i ..
+// 3 i + 2]: the literal, command and distance codes of metablock i, 1 to 256 each, with one literal context; all three 0:
+// the metablock is stored raw.  histos: the counts of every code in code order (256, 704 or 64 words each).  Every split
+// has one block per type, so the header is valid, and every metablock is sized for 256 blocks of each category.  Fills
+// mbs, aux (as k_mb_setup and k_split leave them), the layout, and the image of the whole scratch: the histograms and the
+// splits in place and every other byte `fill`, as a reused arena leaves it.  Returns false on a count out of range.
+#define BR_SYNTH_MB_BYTES (1u << 20)
+static inline bool br_codes_synth(const u32* counts, u32 n, const u32* histos, u8 fill, std::vector<BrMetaBlock>& mbs,
+                                  std::vector<BrMbAux>& aux, BrMbLayout& L, std::vector<u8>& scratch) {
+  BrParams P; memset(&P, 0, sizeof(P));
+  P.n = n * BR_SYNTH_MB_BYTES;
+  mbs.assign(n, BrMetaBlock()); aux.assign(n, BrMbAux());
+  for (u32 i = 0; i < n; ++i) {
+    const u32* c = counts + 3 * i;
+    const bool raw = c[0] == 0 && c[1] == 0 && c[2] == 0;
+    for (int cat = 0; cat < 3; ++cat) if (!raw && (c[cat] < 1 || c[cat] > 256)) return false;
+    BrMetaBlock& mb = mbs[i]; memset(&mb, 0, sizeof(mb));
+    mb.start = i * BR_SYNTH_MB_BYTES; mb.end = mb.start + BR_SYNTH_MB_BYTES;
+    mb.nlit = 254 * 512; mb.ncmd = 254 * 1024;   // br_mb2_nblk: 256, 256 and 510 blocks
+    mb.is_last = i + 1 == n; mb.compress = raw ? 0u : 1u;
+    BrMbAux& a = aux[i]; memset(&a, 0, sizeof(a));
+    if (raw) continue;
+    a.which = 1;
+    u32 off = br_align8((u32)sizeof(BrMbMem));
+    for (int cat = 0; cat < 3; ++cat) {
+      a.num_types[cat] = a.num_blocks[cat] = c[cat];
+      a.var_off[cat] = off; off += br_mb2_var_bytes(br_mb2_nblk(cat, mb.nlit, mb.ncmd));
+    }
+  }
+  br_mb_layout(P, mbs.data(), n, L);
+  scratch.assign(L.scratch_bytes + 256, fill);
+  const u32* h = histos;
+  for (u32 i = 0; i < n; ++i) {
+    if (!mbs[i].compress) continue;
+    const BrMetaBlock& mb = mbs[i]; const BrMbAux& a = aux[i];
+    u8* sc = scratch.data() + L.scratch_off[i];
+    BrMbMem* M = (BrMbMem*)sc;
+    const u32 A[3] = {256, 704, 64};
+    u32* H[3] = {M->lit_H, M->cmd_H, M->dist_H};
+    for (int cat = 0; cat < 3; ++cat) {
+      memcpy(H[cat], h, (size_t)a.num_types[cat] * A[cat] * 4); h += (size_t)a.num_types[cat] * A[cat];
+      const u32 nblk = br_mb2_nblk(cat, mb.nlit, mb.ncmd);
+      u8* types = sc + a.var_off[cat] + nblk * ((u32)sizeof(BrBlockInfo) + 4);
+      u32* lengths = (u32*)(sc + a.var_off[cat] + nblk * (u32)sizeof(BrBlockInfo));
+      for (u32 b = 0; b < a.num_blocks[cat]; ++b) { types[b] = (u8)b; lengths[b] = 1 + 37 * b; }
+    }
+  }
+  return true;
+}
+// Host: what E4 left in the scratch image of br_codes_synth's metablocks.  Per code, in code order: H, depth and bits (256,
+// 704 or 64 entries each).  offsets: per compressed metablock the bit offset of each of its codes (br_mb2_code_bits), then
+// the end of its last code; per raw metablock one 0.
+static inline void br_codes_collect(const std::vector<BrMetaBlock>& mbs, const std::vector<BrMbAux>& aux, const BrMbLayout& L,
+                                    const u8* scratch, u32* H, u8* depth, u16* bits, u32* offsets) {
+  for (size_t i = 0; i < mbs.size(); ++i) {
+    if (!mbs[i].compress) { *offsets++ = 0; continue; }
+    const u8* sc = scratch + L.scratch_off[i];
+    const BrMbMem* M = (const BrMbMem*)sc;
+    const u32 A[3] = {256, 704, 64};
+    const u32* Hs[3] = {M->lit_H, M->cmd_H, M->dist_H};
+    const u8* Ds[3] = {M->lit_depth, M->cmd_depth, M->dist_depth};
+    const u16* Bs[3] = {M->lit_bits, M->cmd_bits, M->dist_bits};
+    u32 ntrees = 0;
+    for (int cat = 0; cat < 3; ++cat) {
+      const size_t k = (size_t)aux[i].num_types[cat] * A[cat];
+      memcpy(H, Hs[cat], k * 4); memcpy(depth, Ds[cat], k); memcpy(bits, Bs[cat], k * 2);
+      H += k; depth += k; bits += k; ntrees += aux[i].num_types[cat];
+    }
+    const u32* code_bits = (const u32*)(sc + br_mb2_scratch_bytes(mbs[i].nlit, mbs[i].ncmd) - BR_CODE_BITS_WORDS * 4);
+    memcpy(offsets, code_bits, (ntrees + 1) * 4ull); offsets += ntrees + 1;
+  }
+}

@@ -597,6 +597,22 @@ extern "C" void* br_job_stream(BrJob* j) { return (void*)j->st; }
 
 static size_t scan_tmp_words(size_t n) { return n / SCAN_CHUNK + n / SCAN_CHUNK / SCAN_CHUNK + 64; }
 
+// E4 (br_entropy2.h): every prefix code of the job built by its own worker, the headers, then every code stored.
+// code_base: n_mbs + 1 words; stmp: scan_tmp_words(n_mbs + 1).  code_ctas: CTAs of thread workers (64 each) when the job
+// has more than BR_CODE_WARP_MAX codes, 0 for L.code_workers of them; tree_pool holds BR_CODE_TREE_NODES for each.
+static u32 codes_ctas(const BrMbLayout& L, u32 code_ctas) { return code_ctas ? code_ctas : (L.code_workers + 63) / 64; }
+static void launch_codes(const BrStream& s, const BrEnt& e, const BrMbLayout& L, u32 n_mbs, u32* code_base, u32* stmp,
+                         BrHTree* tree_pool, u32 code_ctas, cudaStream_t st) {
+  k_code_count<<<(n_mbs + 1 + 255) / 256, 256, 0, st>>>(s, e, code_base, n_mbs);
+  scan_exclusive(code_base, n_mbs + 1, stmp, st);
+  const u32 ctas = L.code_workers ? codes_ctas(L, code_ctas) : 0u;
+  if (L.code_warps) k_codes_warp<false><<<L.code_warps, 32, 0, st>>>(s, e, code_base, n_mbs);
+  if (ctas) k_codes<false><<<ctas, 64, 0, st>>>(s, e, code_base, n_mbs, tree_pool);
+  k_mb_header<<<n_mbs, 32, 0, st>>>(s, e);
+  if (L.code_warps) k_codes_warp<true><<<L.code_warps, 32, 0, st>>>(s, e, code_base, n_mbs);
+  if (ctas) k_codes<true><<<ctas, 64, 0, st>>>(s, e, code_base, n_mbs, tree_pool);
+}
+
 // The position index's arrays and tagS, in arena order; at qualities 2..4 carve_index_quick adds the 32-bit sort arrays.
 static void carve_index(BrCarve& A, const BrParams& P, BrIndexBufs& b) {
   const size_t n = P.n, ntiles = (n + RADIX_TILE - 1) / RADIX_TILE;
@@ -845,15 +861,7 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
       const size_t smem_split = br_split_smem_bytes(256, 13) > br_split_smem_bytes(704, 1) ? br_split_smem_bytes(256, 13) : br_split_smem_bytes(704, 1);
       CK(cudaFuncSetAttribute(k_split, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_split));
       k_split<<<dim3(n_mbs, 3), 256, smem_split, st>>>(s, e);
-      // E4: every prefix code of the job built by its own worker, the headers, then every code stored
-      k_code_count<<<(n_mbs + 1 + 255) / 256, 256, 0, st>>>(s, e, code_base, n_mbs);
-      scan_exclusive(code_base, n_mbs + 1, stmp, st);
-      const u32 code_ctas = (L.code_workers + 63) / 64;
-      if (L.code_warps) k_codes_warp<false><<<L.code_warps, 32, 0, st>>>(s, e, code_base, n_mbs);
-      if (code_ctas) k_codes<false><<<code_ctas, 64, 0, st>>>(s, e, code_base, n_mbs, tree_pool);
-      k_mb_header<<<n_mbs, 32, 0, st>>>(s, e);
-      if (L.code_warps) k_codes_warp<true><<<L.code_warps, 32, 0, st>>>(s, e, code_base, n_mbs);
-      if (code_ctas) k_codes<true><<<code_ctas, 64, 0, st>>>(s, e, code_base, n_mbs, tree_pool);
+      launch_codes(s, e, L, n_mbs, code_base, stmp, tree_pool, 0, st);
     }
     k_lit_bits<<<(e.total_lits + 1 + 255) / 256, 256, 0, st>>>(s, e);
     k_cmd_bits<<<(u32)((C + 1 + 255) / 256), 256, 0, st>>>(s, e);
@@ -1048,6 +1056,64 @@ extern "C" __attribute__((visibility("default"))) int br_debug_search(
   if (h_storedS && cudaMemcpy(h_storedS, storedS, (n + 31) / 32 * 4ull, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
   if (h_prefS && cudaMemcpy(h_prefS, prefS, nsnap * 4ull, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
   ok = nvar;
+done:
+  cudaGetLastError();
+  A.release();
+  return ok;
+}
+
+// Test hook (tests/test_entropy_codes.py): E4 alone, by the pipeline's own launches (launch_codes), on n_mbs synthetic
+// metablocks (br_codes_synth: counts, histos).  The scratch and the thread workers' tree pool start filled with a nonzero
+// pattern, as a reused arena leaves them.  code_ctas: CTAs of thread workers (0: the pipeline's count).  Per code, in code
+// order: H (the smoothed counts), depth, bits (256, 704 or 64 entries each).  offsets: per compressed metablock the bit
+// offset of each of its codes, then the end of its last code; per raw metablock one 0.  out: out_words words of each
+// metablock's bit buffer.  info: the job's codes, the worker kind (1: a warp per code, 2: threads) and the worker count.
+extern "C" __attribute__((visibility("default"))) int br_debug_codes(u32 n_mbs, const u32* h_counts, const u32* h_histos,
+                                                                    u32 code_ctas, u32* h_H, u8* h_depth, u16* h_bits,
+                                                                    u32* h_offsets, u32* h_out, u32 out_words, u32* info) {
+  std::vector<BrMetaBlock> hm; std::vector<BrMbAux> ha; BrMbLayout L; std::vector<u8> img;
+  if (n_mbs == 0 || !br_codes_synth(h_counts, n_mbs, h_histos, 0xA5, hm, ha, L, img)) return 0;
+  BrDeviceTables* T = get_tables();
+  if (!T) return 0;
+  BrStream s; memset(&s, 0, sizeof(s));
+  s.P.n = n_mbs * BR_SYNTH_MB_BYTES;
+  br_bind_tables(s, T->blob, T->log2tab, T->log2tab_n);
+  BrEnt e; memset(&e, 0, sizeof(e));
+  const u32 ctas = L.code_workers ? codes_ctas(L, code_ctas) : 0u;
+  u64 *soff, *ooff; u32 *code_base, *stmp; BrHTree* pool;
+  auto carve = [&](BrCarve& A) {
+    e.scratch = A.take<u8>(img.size()); e.outbits = A.take<u32>(L.out_words + 64);
+    e.scratch_off = soff = A.take<u64>(n_mbs); e.out_off = ooff = A.take<u64>(n_mbs);
+    e.aux = A.take<BrMbAux>(n_mbs); s.mbs = A.take<BrMetaBlock>(n_mbs);
+    code_base = A.take<u32>(n_mbs + 1); stmp = A.take<u32>(scan_tmp_words(n_mbs + 1) * 2);
+    pool = A.take<BrHTree>((size_t)ctas * 64 * BR_CODE_TREE_NODES + 1);
+  };
+  BrArena A;
+  if (!br_carve(A, carve)) return 0;
+  int ok = 0;
+  u32 total = 0;
+  std::vector<u8> sc;
+  if (cudaMemcpy(e.scratch, img.data(), img.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemset(e.outbits, 0, (L.out_words + 64) * 4) != cudaSuccess ||
+      cudaMemcpy(soff, L.scratch_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(ooff, L.out_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(e.aux, ha.data(), n_mbs * sizeof(BrMbAux), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy((BrMetaBlock*)s.mbs, hm.data(), n_mbs * sizeof(BrMetaBlock), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemset(pool, 0xA5, ((size_t)ctas * 64 * BR_CODE_TREE_NODES + 1) * sizeof(BrHTree)) != cudaSuccess) goto done;
+  launch_codes(s, e, L, n_mbs, code_base, stmp, pool, code_ctas, 0);
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(&total, code_base + n_mbs, 4, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  sc.resize(img.size());
+  if (cudaMemcpy(sc.data(), e.scratch, img.size(), cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  for (u32 i = 0; i < n_mbs; ++i) {
+    if (hm[i].compress &&
+        cudaMemcpy(h_out + (size_t)i * out_words, e.outbits + L.out_off[i],
+                   4ull * (i + 1 < n_mbs ? L.out_off[i + 1] - L.out_off[i] < out_words ? L.out_off[i + 1] - L.out_off[i] : out_words
+                                         : L.out_words - L.out_off[i] < out_words ? L.out_words - L.out_off[i] : out_words),
+                   cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  }
+  br_codes_collect(hm, ha, L, sc.data(), h_H, h_depth, h_bits, h_offsets);
+  info[0] = total; info[1] = total > BR_CODE_WARP_MAX ? 2u : 1u; info[2] = total > BR_CODE_WARP_MAX ? ctas * 64 : total;
+  ok = 1;
 done:
   cudaGetLastError();
   A.release();

@@ -66,6 +66,10 @@ double oracle_fast_log2(size_t v) { return fast_log2(v); }
  *       split reached the 256 / nc type cap; split_back: blocks merged into the type before last (action 2)
  *   max_lit_types / max_lit_trees / max_cmd_types / max_dist_types: per metablock
  *   max_insert / max_copy / max_block_len / max_distance: the longest emitted (distance: explicit codes only)
+ *   codes: the literal, command and distance prefix codes stored by compressed metablocks, summed
+ *   rle_good / rle_stride: smoothed histograms with runs marked good_for_rle / with a stride of counts averaged
+ *   cl_single: code-length codes of one symbol (stored with zero bits); cl_skip2 / cl_skip3: HSKIP 2 / 3;
+ *       cl_trim: code-length codes whose trailing zero lengths are left out
  * The same for the match search (find_longest_match, tests/test_search_probe.py):
  *   srch_dc_len2: searches won by a len-2 distance-cache match; srch_ring_break: the ring-buffer stop
  *       (cur_m + best_len > rmask); srch_ring_skip: a candidate skipped by prev_m + best_len > rmask;
@@ -76,11 +80,12 @@ double oracle_fast_log2(size_t v) { return fast_log2(v); }
   X(simple_nsym1) X(simple_nsym2) X(simple_nsym3) X(simple_nsym4) X(simple_select0) X(simple_select1) X(rle_lt16) X(rle_lt28) X(rle_full) X(rle_holes) \
   X(reps7) X(reps11) X(rle_use_nz) X(rle_use_z) X(ctx_nc1) X(ctx_nc2) X(ctx_nc3) X(ctx_nc13) X(lit_cap_nc1) \
   X(lit_cap_nc2) X(lit_cap_nc3) X(lit_cap_nc13) X(split_back) X(max_lit_types) X(max_lit_trees) X(max_cmd_types) \
-  X(max_dist_types) X(max_insert) X(max_copy) X(max_block_len) X(max_distance) \
+  X(max_dist_types) X(max_insert) X(max_copy) X(max_block_len) X(max_distance) X(codes) \
+  X(rle_good) X(rle_stride) X(cl_single) X(cl_skip2) X(cl_skip3) X(cl_trim) \
   X(srch_dc_len2) X(srch_ring_break) X(srch_ring_skip) X(srch_tie_max) X(srch_wrap_cut) X(srch_dict_hit) X(srch_gate_closed)
 #define EDGE_MEMBER(f) uint64_t f;
 #define EDGE_NAME(f) #f ","
-static struct { EDGE_FIELDS(EDGE_MEMBER) } g_edge;
+static _Thread_local struct { EDGE_FIELDS(EDGE_MEMBER) } g_edge;   /* per thread: callers may run the oracle in a pool */
 #define EDGE_MAX(f, v) do { if ((uint64_t)(v) > g_edge.f) g_edge.f = (uint64_t)(v); } while (0)
 void oracle_edge_stats_reset(void) { memset(&g_edge, 0, sizeof(g_edge)); }
 /* The counters as uint64 words in the order of oracle_edge_stats_names(); returns how many there are. */
@@ -757,6 +762,7 @@ static void optimize_counts_for_rle(size_t length, uint32_t* counts, uint8_t* go
       if (i == length || counts[i] != symbol) {
         if ((symbol == 0 && step >= 5) || (symbol != 0 && step >= 7)) {
           size_t k; for (k = 0; k < step; ++k) good_for_rle[i - k - 1] = 1;
+          ++g_edge.rle_good;
         }
         step = 1;
         if (i != length) symbol = counts[i];
@@ -774,6 +780,7 @@ static void optimize_counts_for_rle(size_t length, uint32_t* counts, uint8_t* go
         if (count == 0) count = 1;
         if (sum == 0) count = 0;
         for (k = 0; k < stride; ++k) counts[i - k - 1] = (uint32_t)count;
+        ++g_edge.rle_stride;
       }
       stride = 0; sum = 0;
       if (i < length - 2) limit = (uint32_t)(256u * (counts[i] + counts[i + 1] + counts[i + 2]) / 3u + 420u);
@@ -867,6 +874,8 @@ static void store_hufftree_of_hufftree(int num_codes, const uint8_t* cl_depth, B
     skip = 2;
     if (cl_depth[kOrder[2]] == 0) skip = 3;
   }
+  if (skip == 2) ++g_edge.cl_skip2; else if (skip == 3) ++g_edge.cl_skip3;
+  if (to_store < 18) ++g_edge.cl_trim;
   wbits(w, 2, skip);
   for (i = skip; i < to_store; ++i) { size_t l = cl_depth[kOrder[i]]; wbits(w, kLen[l], kSym[l]); }
 }
@@ -886,7 +895,7 @@ static void store_huffman_tree(const uint8_t* depths, size_t num, HTree* tree, B
   create_huffman_tree(histo, 18, 5, tree, cl_depth);
   depths_to_symbols(cl_depth, 18, cl_bits);
   store_hufftree_of_hufftree(num_codes, cl_depth, w);
-  if (num_codes == 1) cl_depth[code] = 0;
+  if (num_codes == 1) { cl_depth[code] = 0; ++g_edge.cl_single; }
   for (i = 0; i < hs; ++i) {
     size_t ix = ht[i];
     wbits(w, cl_depth[ix], cl_bits[ix]);
@@ -932,6 +941,29 @@ static void build_and_store_tree(const uint32_t* histo, size_t histo_len, size_t
   depths_to_symbols(depth, histo_len, bits);
   if (count <= 4) store_simple_tree(depth, s4, count, max_bits, w);
   else store_huffman_tree(depth, histo_len, tree, w);
+}
+
+/* One prefix code of a metablock of quality 4+, with exactly the calls store_compressed_metablock makes for it: the count
+   smoothing, then the Huffman construction and the store into a fresh bit writer.  histo: len (256, 704 or 64) counts.
+   H_out: the smoothed counts; depth_out / bits_out: zero, then what build_and_store_tree writes (with one symbol or none
+   only that symbol's entry); stored: the code's bits, stored_cap bytes; *nbits: its size in bits.  Returns 0 when len is
+   not an alphabet size of such a metablock or the code does not fit stored_cap. */
+int oracle_build_code(const uint32_t* histo, size_t len, uint32_t* H_out, uint8_t* depth_out, uint16_t* bits_out,
+                      uint8_t* stored, size_t stored_cap, size_t* nbits) {
+  uint8_t good_for_rle[704];
+  HTree* tree; BitW w; size_t nbytes;
+  if (len != 256 && len != 704 && len != 64) return 0;
+  tree = (HTree*)malloc(sizeof(HTree) * (2 * 704 + 1));
+  w.buf = (uint8_t*)calloc(2 * len + 256, 1); w.ix = 0;   /* (at most 8 bits a code length, and the code-length code) */
+  memcpy(H_out, histo, len * 4);
+  memset(depth_out, 0, len); memset(bits_out, 0, len * 2);
+  optimize_counts_for_rle(len, H_out, good_for_rle);
+  build_and_store_tree(H_out, len, len, tree, depth_out, bits_out, &w);
+  *nbits = w.ix;
+  nbytes = (w.ix + 7) / 8;
+  if (nbytes <= stored_cap) memcpy(stored, w.buf, nbytes);
+  free(w.buf); free(tree);
+  return nbytes <= stored_cap;
 }
 
 /* brotli_bit_stream.c:106 */
@@ -1398,6 +1430,7 @@ static void store_compressed_metablock(Enc* e, size_t start_pos, size_t length,
     else ++g_edge.lit_cap_nc13;
   }
   EDGE_MAX(max_lit_types, lit_split.num_types); EDGE_MAX(max_lit_trees, ls.histograms_size);
+  g_edge.codes += ls.histograms_size + cs.histograms_size + ds.histograms_size;
   EDGE_MAX(max_cmd_types, cmd_split.num_types); EDGE_MAX(max_dist_types, dist_split.num_types);
   { const Split* sp[3] = {&lit_split, &cmd_split, &dist_split}; size_t k;   /* lengths are stored with 2+ types only */
     for (k = 0; k < 3; ++k)
@@ -1632,6 +1665,7 @@ static void store_metablock_fast_trivial(Enc* e, size_t start_pos, size_t length
   uint16_t lit_bits[256], cmd_bits[704], dist_bits[140];
   HTree* tree = (HTree*)malloc(sizeof(HTree) * (2 * 704 + 1));
   size_t i, pos = start_pos, nlit = 0, ndist = 0;
+  g_edge.codes += 3;
   memset(lit_histo, 0, sizeof(lit_histo)); memset(cmd_histo, 0, sizeof(cmd_histo)); memset(dist_histo, 0, sizeof(dist_histo));
   memset(lit_depth, 0, sizeof(lit_depth)); memset(cmd_depth, 0, sizeof(cmd_depth)); memset(dist_depth, 0, sizeof(dist_depth));
   memset(lit_bits, 0, sizeof(lit_bits)); memset(cmd_bits, 0, sizeof(cmd_bits)); memset(dist_bits, 0, sizeof(dist_bits));

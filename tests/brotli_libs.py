@@ -112,6 +112,27 @@ class Oracle:
         assert len(names) == n
         return dict(zip(names, vals))
 
+    def stored_codes(self):
+        """The literal, command and distance prefix codes stored by compressed metablocks since the last edge_stats_reset()."""
+        return self.edge_stats()["codes"]
+
+    def build_code(self, histo):
+        """One prefix code as a metablock of quality 4+ builds and stores it (oracle_build_code): the smoothed counts, the
+        depths, the code words, the stored bits (bytes, LSB first) and their number.  histo: 256, 704 or 64 counts."""
+        import numpy as np
+        L = self.lib
+        L.oracle_build_code.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                        C.POINTER(C.c_size_t)]
+        L.oracle_build_code.restype = C.c_int
+        h = np.ascontiguousarray(histo, np.uint32)
+        n = len(h)
+        H, depth, bits = np.zeros(n, np.uint32), np.zeros(n, np.uint8), np.zeros(n, np.uint16)
+        stored = C.create_string_buffer(2 * n + 256)
+        nbits = C.c_size_t(0)
+        assert L.oracle_build_code(h.ctypes.data, n, H.ctypes.data, depth.ctypes.data, bits.ctypes.data, stored, len(stored),
+                                   C.byref(nbits)) == 1, n
+        return H, depth, bits, stored.raw[:(nbits.value + 7) // 8], nbits.value
+
     def compress(self, data, quality, lgwin):
         n = len(data)
         cap = n + (n >> 1) + 4096

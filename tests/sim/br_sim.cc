@@ -532,6 +532,51 @@ extern "C" long sim_compress_cuts(int q, int lgwin, u32 size_hint, const u8* in,
   const BrCuts c = {cut_pos, cut_kind, ncuts, is_final, with_header, finish_empty, end_bit, lgblock, disable_ctx, stream_offset, nullptr};
   return sim_compress_impl(q, lgwin, size_hint, in, n, out, out_cap, stats, &c);
 }
+
+// E4 alone on synthetic metablocks: the counterpart of the product's br_debug_codes hook, with its arguments.  A job of at
+// most BR_CODE_WARP_MAX codes takes the warp workers' functions with one lane, as br_prep_codes does; a larger one the
+// thread workers' functions over a pool of tree areas, each worker taking the codes k_codes gives it, in its order.  The
+// scratch, the warps' shared copy and the tree areas start with the device hook's pattern.
+extern "C" int sim_debug_codes(u32 n_mbs, const u32* counts, const u32* histos, u32 code_ctas, u32* H, u8* depth, u16* bits,
+                               u32* offsets, u32* out, u32 out_words, u32* info) {
+  std::vector<BrMetaBlock> mbs; std::vector<BrMbAux> aux; BrMbLayout L; std::vector<u8> sc;
+  if (n_mbs == 0 || !br_codes_synth(counts, n_mbs, histos, 0xA5, mbs, aux, L, sc)) return 0;
+  BrStream s; memset(&s, 0, sizeof(s));
+  s.P.n = n_mbs * BR_SYNTH_MB_BYTES; s.mbs = mbs.data();
+  br_bind_tables(s, g_t.blob.data(), g_t.log2tab.data(), (u32)g_t.log2tab.size());
+  std::vector<u32> outbits(L.out_words + 64, 0), code_base(n_mbs + 1, 0);
+  for (u32 i = 0; i < n_mbs; ++i) code_base[i + 1] = code_base[i] + (mbs[i].compress ? br_mb_code_count(aux[i]) : 0u);   // k_code_count + scan
+  const u32 total = code_base[n_mbs];
+  const bool warps = total <= BR_CODE_WARP_MAX;
+  const u32 nwk = warps ? total : (code_ctas ? code_ctas : (L.code_workers + 63) / 64) * 64;
+  std::vector<BrHTree> pool(warps ? 1 : (size_t)nwk * BR_CODE_TREE_NODES);
+  memset(pool.data(), 0xA5, pool.size() * sizeof(BrHTree));
+  std::vector<u8> smem(sizeof(BrCodeSmem), 0xA5);
+  BrCodeSmem* S = (BrCodeSmem*)smem.data();
+  auto code = [&](u32 t, u32 wk, bool store) {
+    const u32 m = br_upper_index(code_base.data(), n_mbs, t);
+    u8* msc = sc.data() + L.scratch_off[m];
+    u32* mout = outbits.data() + L.out_off[m];
+    if (warps) { if (store) br_code_store_warp(mbs[m], aux[m], msc, t - code_base[m], S, mout); else br_code_build_warp(mbs[m], aux[m], msc, t - code_base[m], S); }
+    else { BrHTree* tree = pool.data() + (size_t)wk * BR_CODE_TREE_NODES;
+           if (store) br_code_store(mbs[m], aux[m], msc, t - code_base[m], tree, mout); else br_code_build(mbs[m], aux[m], msc, t - code_base[m], tree); }
+  };
+  for (int store = 0; store < 2; ++store) {
+    if (store)
+      for (u32 i = 0; i < n_mbs; ++i)
+        if (mbs[i].compress) br_mb_header(s, mbs[i], aux[i], sc.data() + L.scratch_off[i], outbits.data() + L.out_off[i]);
+    for (u32 wk = 0; wk < nwk; ++wk)
+      for (u32 t = wk; t < total; t += nwk) code(t, wk, store != 0);
+  }
+  br_codes_collect(mbs, aux, L, sc.data(), H, depth, bits, offsets);
+  for (u32 i = 0; i < n_mbs; ++i) {
+    if (!mbs[i].compress) continue;
+    const size_t have = (i + 1 < n_mbs ? L.out_off[i + 1] : L.out_words) - L.out_off[i];
+    memcpy(out + (size_t)i * out_words, outbits.data() + L.out_off[i], 4 * std::min<size_t>(have, out_words));
+  }
+  info[0] = total; info[1] = warps ? 1u : 2u; info[2] = nwk;
+  return 1;
+}
 #endif
 
 // ------------------------------------------------------------------ quality 1 (br_q1.h)
