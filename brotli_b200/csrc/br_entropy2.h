@@ -145,6 +145,33 @@ BR_DEV void br_expand_cmds(const BrEnt& e, u32 first_cmd) {
   }
 }
 
+// ---------------------------------------------------------------------------------- E2 / E3 setup
+// What k_mb_setup records for a compressed metablock once E2 has chosen `which`: its first literal and distance ordinals,
+// its symbol counts and where its block arrays lie in the scratch.
+BR_DEV void br_mb_aux_init(BrMbAux& a, const BrMetaBlock& mb, const BrEnt& e, u32 which) {
+  memset(&a, 0, sizeof(a));
+  a.which = which;
+  a.lit_base = e.lit_ord[mb.cmd_off]; a.dist_base = e.dist_ord[mb.cmd_off];
+  a.nsym[0] = mb.nlit; a.nsym[1] = mb.ncmd; a.nsym[2] = e.dist_ord[mb.cmd_off + mb.ncmd] - a.dist_base;
+  u32 off = br_align8((u32)sizeof(BrMbMem));
+  for (int cat = 0; cat < 3; ++cat) { a.var_off[cat] = off; off += br_mb2_var_bytes(br_mb2_nblk(cat, mb.nlit, mb.ncmd)); }
+}
+// The greedy splitter's constants of a category (metablock.c:708): alphabet, histogram contexts (literals, cat 0, have
+// the metablock's `which`; commands and distances one), shortest block and split threshold.  Macros, so that k_split
+// reads `which` only for literals, as it always has; br_split_cat gathers them for the CPU simulation.
+#define BR_SPLIT_ALPHABET(cat) ((cat) == 0 ? 256u : (cat) == 1 ? 704u : 64u)
+#define BR_SPLIT_CONTEXTS(cat, which) ((cat) == 0 ? (which) : 1u)
+#define BR_SPLIT_MIN_BLOCK(cat) ((cat) == 1 ? 1024u : 512u)
+#define BR_SPLIT_THR(cat) ((cat) == 0 ? 400.0 : (cat) == 1 ? 500.0 : 100.0)
+#define BR_SPLIT_HIST(M, cat) ((cat) == 0 ? (M)->lit_H : (cat) == 1 ? (M)->cmd_H : (M)->dist_H)
+struct BrSplitCat { u32 A, nc, min_block; double thr; };
+BR_HD BrSplitCat br_split_cat(int cat, u32 which) {
+  BrSplitCat k;
+  k.A = BR_SPLIT_ALPHABET(cat); k.nc = BR_SPLIT_CONTEXTS(cat, which);
+  k.min_block = BR_SPLIT_MIN_BLOCK(cat); k.thr = BR_SPLIT_THR(cat);
+  return k;
+}
+
 // ---------------------------------------------------------------------------------- E3
 struct BrSplitState {
   u32 target, block_size, num_blocks, num_types, last_ix[2], merge_last_count, action;
@@ -734,4 +761,68 @@ static inline void br_codes_collect(const std::vector<BrMetaBlock>& mbs, const s
     const u32* code_bits = (const u32*)(sc + br_mb2_scratch_bytes(mbs[i].nlit, mbs[i].ncmd) - BR_CODE_BITS_WORDS * 4);
     memcpy(offsets, code_bits, (ntrees + 1) * 4ull); offsets += ntrees + 1;
   }
+}
+
+// Host: metablocks for E2..E4 described by the caller (the test hooks br_debug_split and tests/sim sim_debug_split).
+// mbw: BR_SPLIT_MB_WORDS words per metablock: start, end, first command, command count, is_last, compress (0: stored
+// raw) and base, the first byte of its stream (literal contexts see zeros in front of it).  The metablocks and their
+// commands must cover the n input bytes in order, as the compacted commands of a job do.  Fills mbs (nlit from the
+// commands) and the layout; returns false on a description that does not hold together.
+#define BR_SPLIT_MB_WORDS 7
+static inline bool br_split_synth(const BrParams& P, const u32* mbw, u32 n_mbs, const BrCmd* cmds, u32 ncmd,
+                                  std::vector<BrMetaBlock>& mbs, BrMbLayout& L) {
+  mbs.assign(n_mbs, BrMetaBlock());
+  u32 pos = 0, c = 0;
+  for (u32 i = 0; i < n_mbs; ++i) {
+    const u32* w = mbw + (size_t)i * BR_SPLIT_MB_WORDS;
+    BrMetaBlock& mb = mbs[i]; memset(&mb, 0, sizeof(mb));
+    mb.start = w[0]; mb.end = w[1]; mb.cmd_off = w[2]; mb.ncmd = w[3]; mb.is_last = w[4]; mb.compress = w[5]; mb.base = w[6];
+    if (mb.start != pos || mb.end <= mb.start || mb.cmd_off != c || mb.ncmd == 0 || (u64)c + mb.ncmd > ncmd || mb.base > mb.start)
+      return false;
+    u64 span = 0;
+    for (u32 k = c; k < c + mb.ncmd; ++k) { mb.nlit += cmds[k].insert_len; span += (u64)cmds[k].insert_len + (cmds[k].copy_len & 0x1FFFFFF); }
+    if (span != mb.end - mb.start) return false;
+    pos = mb.end; c += mb.ncmd;
+  }
+  if (pos != P.n || c != ncmd) return false;
+  br_mb_layout(P, mbs.data(), n_mbs, L);
+  return true;
+}
+// Host: the record of a compressed metablock that the split hooks return, from the image of its scratch after E3 (before
+// E4 smooths the histograms in place): which, num_types[3], num_blocks[3], a word for the bit count (br_split_record_bits),
+// then per category types[num_blocks] and lengths[num_blocks] (a word each), then the histograms: literal (num_types *
+// which rows of 256), command (rows of 704) and distance (rows of 64).
+#define BR_SPLIT_REC_HEAD 8
+static inline void br_split_record(const BrMetaBlock& mb, const BrMbAux& a, const u8* sc, std::vector<u32>& rec) {
+  rec.assign({a.which, a.num_types[0], a.num_types[1], a.num_types[2], a.num_blocks[0], a.num_blocks[1], a.num_blocks[2], 0u});
+  for (int cat = 0; cat < 3; ++cat) {
+    const u32 nblk = br_mb2_nblk(cat, mb.nlit, mb.ncmd);
+    const u8* types = sc + a.var_off[cat] + nblk * ((u32)sizeof(BrBlockInfo) + 4);
+    const u32* lengths = (const u32*)(sc + a.var_off[cat] + nblk * (u32)sizeof(BrBlockInfo));
+    for (u32 b = 0; b < a.num_blocks[cat]; ++b) rec.push_back(types[b]);
+    rec.insert(rec.end(), lengths, lengths + a.num_blocks[cat]);
+  }
+  const BrMbMem* M = (const BrMbMem*)sc;
+  rec.insert(rec.end(), M->lit_H, M->lit_H + (size_t)a.num_types[0] * a.which * 256);
+  rec.insert(rec.end(), M->cmd_H, M->cmd_H + (size_t)a.num_types[1] * 704);
+  rec.insert(rec.end(), M->dist_H, M->dist_H + (size_t)a.num_types[2] * 64);
+}
+// ... then, after E4, the metablock's bit buffer from bit 0 to the end of its last prefix code: the header, the block-split
+// codes, the context maps and every code (nbits bits, (nbits + 31) / 32 words).
+static inline void br_split_record_bits(std::vector<u32>& rec, const u32* bits, u32 nbits) {
+  rec[7] = nbits;
+  rec.insert(rec.end(), bits, bits + (nbits + 31) / 32);
+}
+// The offset in the scratch of a metablock's code bit offsets (br_mb2_code_bits); entry br_mb_code_count(a) is the end of
+// its last code.
+static inline size_t br_split_code_end_off(const BrMetaBlock& mb, const BrMbAux& a) {
+  return br_mb2_scratch_bytes(mb.nlit, mb.ncmd) - BR_CODE_BITS_WORDS * 4 + 4ull * (a.num_types[0] * a.which + a.num_types[1] + a.num_types[2]);
+}
+// The records of every compressed metablock, one after another, into out (cap words).  Returns the words they take.
+static inline size_t br_split_put(const std::vector<std::vector<u32>>& recs, u32* out, size_t cap) {
+  size_t k = 0;
+  for (const auto& r : recs) {
+    for (size_t j = 0; j < r.size(); ++j, ++k) if (k < cap) out[k] = r[j];
+  }
+  return k;
 }

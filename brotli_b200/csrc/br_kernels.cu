@@ -373,12 +373,8 @@ __global__ void __launch_bounds__(32) k_mb_setup(BrStream s, BrEnt e) {
   BrMbMem* M = (BrMbMem*)sc;
   u32 which = s.P.disable_ctx ? 1u : br_decide_context_modeling(s, mb.start, mb.end - mb.start, M->sc.rle_syms);
   if (threadIdx.x == 0) {
-    BrMbAux a; memset(&a, 0, sizeof(a));
-    a.which = which;
-    a.lit_base = e.lit_ord[mb.cmd_off]; a.dist_base = e.dist_ord[mb.cmd_off];
-    a.nsym[0] = mb.nlit; a.nsym[1] = mb.ncmd; a.nsym[2] = e.dist_ord[mb.cmd_off + mb.ncmd] - a.dist_base;
-    u32 off = br_align8((u32)sizeof(BrMbMem));
-    for (int cat = 0; cat < 3; ++cat) { a.var_off[cat] = off; off += br_mb2_var_bytes(br_mb2_nblk(cat, mb.nlit, mb.ncmd)); }
+    BrMbAux a;
+    br_mb_aux_init(a, mb, e, which);
     e.aux[i] = a;
   }
 }
@@ -390,10 +386,10 @@ __global__ void __launch_bounds__(256) k_split(BrStream s, BrEnt e) {
   BrMbAux& a = e.aux[i];
   u8* sc = e.scratch + e.scratch_off[i];
   BrMbMem* M = (BrMbMem*)sc;
-  const u32 A = cat == 0 ? 256u : cat == 1 ? 704u : 64u, nc = cat == 0 ? a.which : 1u;
-  const u32 minb = cat == 1 ? 1024u : 512u;
-  const double thr = cat == 0 ? 400.0 : cat == 1 ? 500.0 : 100.0;
-  u32* H = cat == 0 ? M->lit_H : cat == 1 ? M->cmd_H : M->dist_H;
+  const u32 A = BR_SPLIT_ALPHABET(cat), nc = BR_SPLIT_CONTEXTS(cat, a.which);
+  const u32 minb = BR_SPLIT_MIN_BLOCK(cat);
+  const double thr = BR_SPLIT_THR(cat);
+  u32* H = BR_SPLIT_HIST(M, cat);
   u32 nblk = br_mb2_nblk(cat, mb.nlit, mb.ncmd);
   br_split_cta(s, e, mb, a, cat, A, nc, minb, thr, a.nsym[cat], br_mb2_types(sc, a, cat, nblk),
                br_mb2_lengths(sc, a, cat, nblk), H, sm);
@@ -611,6 +607,16 @@ static void launch_codes(const BrStream& s, const BrEnt& e, const BrMbLayout& L,
   k_mb_header<<<n_mbs, 32, 0, st>>>(s, e);
   if (L.code_warps) k_codes_warp<true><<<L.code_warps, 32, 0, st>>>(s, e, code_base, n_mbs);
   if (ctas) k_codes<true><<<ctas, 64, 0, st>>>(s, e, code_base, n_mbs, tree_pool);
+}
+// E2 (the literal context decision and the metablock's BrMbAux) and, at qualities 4..9, E3 (the block splits and their
+// histograms): what launch_codes starts from.  Returns false on a CUDA error.
+static bool launch_split(const BrStream& s, const BrEnt& e, u32 n_mbs, cudaStream_t st) {
+  k_mb_setup<<<n_mbs, 32, 0, st>>>(s, e);
+  if (s.P.mb_kind) return true;
+  const size_t smem_split = br_split_smem_bytes(256, 13) > br_split_smem_bytes(704, 1) ? br_split_smem_bytes(256, 13) : br_split_smem_bytes(704, 1);
+  CK(cudaFuncSetAttribute(k_split, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_split));
+  k_split<<<dim3(n_mbs, 3), 256, smem_split, st>>>(s, e);
+  return true;
 }
 
 // The position index's arrays and tagS, in arena order; at qualities 2..4 carve_index_quick adds the 32-bit sort arrays.
@@ -855,14 +861,9 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
     const u32 grid_mbs = n_mbs < 65535u ? n_mbs : 65535u;
     k_cmd_mb<<<dim3(64, grid_mbs), 256, 0, st>>>(s, e.cmd_mb, n_mbs);
     k_expand<<<(u32)((C + 127) / 128 + 1), 128, 0, st>>>(e);
-    k_mb_setup<<<n_mbs, 32, 0, st>>>(s, e);
+    if (!launch_split(s, e, n_mbs, st)) return 0;
     if (P.mb_kind) k_prep_flat<<<n_mbs, 64, 0, st>>>(s, e);   // qualities 2, 3: no block split, one code per category
-    else {
-      const size_t smem_split = br_split_smem_bytes(256, 13) > br_split_smem_bytes(704, 1) ? br_split_smem_bytes(256, 13) : br_split_smem_bytes(704, 1);
-      CK(cudaFuncSetAttribute(k_split, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_split));
-      k_split<<<dim3(n_mbs, 3), 256, smem_split, st>>>(s, e);
-      launch_codes(s, e, L, n_mbs, code_base, stmp, tree_pool, 0, st);
-    }
+    else launch_codes(s, e, L, n_mbs, code_base, stmp, tree_pool, 0, st);
     k_lit_bits<<<(e.total_lits + 1 + 255) / 256, 256, 0, st>>>(s, e);
     k_cmd_bits<<<(u32)((C + 1 + 255) / 256), 256, 0, st>>>(s, e);
     scan_exclusive(e.lit_len, e.total_lits + 1, stmp, st);
@@ -1118,4 +1119,85 @@ done:
   cudaGetLastError();
   A.release();
   return ok;
+}
+
+// Test hook (tests/test_entropy_split.py): E0..E4 on metablocks the caller describes (br_split_synth: n input bytes, ncmd
+// commands of 16 bytes, BR_SPLIT_MB_WORDS words per metablock), by the pipeline's own launches: the E0 scans, k_expand,
+// launch_split and launch_codes.  The scratch starts filled with a nonzero pattern, as a reused arena leaves it.  Writes
+// the records of the compressed metablocks (br_split_record, br_split_record_bits) to out, at most out_cap words, and
+// returns the words they take (0: failure); no symbol is coded and nothing is assembled.
+extern "C" __attribute__((visibility("default"))) long br_debug_split(const u8* h_in, u32 n, const BrCmd* h_cmds, u32 ncmd,
+                                                                     const u32* h_mbs, u32 n_mbs, int quality, u32 size_hint,
+                                                                     int disable_ctx, u32* h_out, size_t out_cap) {
+  if (n == 0 || n_mbs == 0 || quality < 4 || quality > 9) return 0;
+  BrStream s; memset(&s, 0, sizeof(s));
+  s.P.quality = quality; s.P.n = n; s.P.size_hint = size_hint; s.P.disable_ctx = disable_ctx ? 1u : 0u;
+  std::vector<BrMetaBlock> hm; BrMbLayout L;
+  if (!br_split_synth(s.P, h_mbs, n_mbs, h_cmds, ncmd, hm, L)) return 0;
+  BrDeviceTables* T = get_tables();
+  if (!T) return 0;
+  br_bind_tables(s, T->blob, T->log2tab, T->log2tab_n);
+  u32 total_lits = 0, total_dist = 0;
+  for (u32 i = 0; i < ncmd; ++i) {
+    total_lits += h_cmds[i].insert_len; total_dist += (h_cmds[i].copy_len & 0x1FFFFFF) && h_cmds[i].cmd_prefix >= 128;
+  }
+  BrEnt e; memset(&e, 0, sizeof(e));
+  e.total_cmds = ncmd; e.total_lits = total_lits; e.total_dist = total_dist;
+  u64 *soff, *ooff; u32 *lit_ord, *cmd_pos, *dist_ord, *code_base, *stmp; BrHTree* pool;
+  const size_t pool_nodes = (size_t)((L.code_workers + 63) & ~63u) * BR_CODE_TREE_NODES + 1;
+  auto carve = [&](BrCarve& A) {
+    s.data = A.take<u8>((size_t)n + 64); e.cmds = A.take<BrCmd>(ncmd + 1);
+    e.lit_ord = lit_ord = A.take<u32>(ncmd + 2); e.cmd_pos = cmd_pos = A.take<u32>(ncmd + 2); e.dist_ord = dist_ord = A.take<u32>(ncmd + 2);
+    e.lit_pos = A.take<u32>(total_lits + 2); e.lit_cmd = A.take<u32>(total_lits + 2); e.dist_sym = A.take<u16>(ncmd + 2);
+    e.scratch = A.take<u8>(L.scratch_bytes + 256); e.outbits = A.take<u32>(L.out_words + 64);
+    e.scratch_off = soff = A.take<u64>(n_mbs); e.out_off = ooff = A.take<u64>(n_mbs);
+    e.aux = A.take<BrMbAux>(n_mbs); s.mbs = A.take<BrMetaBlock>(n_mbs);
+    code_base = A.take<u32>(n_mbs + 1); stmp = A.take<u32>(scan_tmp_words((size_t)n + ncmd + 8) * 2);
+    pool = A.take<BrHTree>(pool_nodes);
+  };
+  BrArena A;
+  if (!br_carve(A, carve)) return 0;
+  long ret = 0;
+  std::vector<BrMbAux> ha(n_mbs);
+  std::vector<std::vector<u32>> recs;
+  std::vector<u8> img;
+  if (cudaMemset((u8*)s.data, 0, (size_t)n + 64) != cudaSuccess || cudaMemcpy((u8*)s.data, h_in, n, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy((BrCmd*)e.cmds, h_cmds, ncmd * sizeof(BrCmd), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemset(e.scratch, 0xA5, L.scratch_bytes + 256) != cudaSuccess ||
+      cudaMemset(e.outbits, 0, (L.out_words + 64) * 4) != cudaSuccess ||
+      cudaMemcpy(soff, L.scratch_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(ooff, L.out_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy((BrMetaBlock*)s.mbs, hm.data(), n_mbs * sizeof(BrMetaBlock), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemset(pool, 0xA5, pool_nodes * sizeof(BrHTree)) != cudaSuccess) goto done;
+  // E0 and E1 as job_compress runs them
+  k_cmd_scan_inputs<<<(ncmd + 1 + 255) / 256, 256>>>(e.cmds, ncmd, lit_ord, cmd_pos, dist_ord);
+  scan_exclusive(lit_ord, ncmd + 1, stmp, 0);
+  scan_exclusive(cmd_pos, ncmd + 1, stmp, 0);
+  scan_exclusive(dist_ord, ncmd + 1, stmp, 0);
+  k_expand<<<(ncmd + 127) / 128 + 1, 128>>>(e);
+  if (!launch_split(s, e, n_mbs, 0) || cudaDeviceSynchronize() != cudaSuccess ||
+      cudaMemcpy(ha.data(), e.aux, n_mbs * sizeof(BrMbAux), cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  for (u32 i = 0; i < n_mbs; ++i) {   // the splits and histograms before E4 smooths them
+    if (!hm[i].compress) continue;
+    img.resize(br_mb2_scratch_bytes(hm[i].nlit, hm[i].ncmd));
+    if (cudaMemcpy(img.data(), e.scratch + L.scratch_off[i], img.size(), cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+    recs.emplace_back();
+    br_split_record(hm[i], ha[i], img.data(), recs.back());
+  }
+  launch_codes(s, e, L, n_mbs, code_base, stmp, pool, 0, 0);
+  if (cudaDeviceSynchronize() != cudaSuccess) goto done;
+  for (u32 i = 0, r = 0; i < n_mbs; ++i) {
+    if (!hm[i].compress) continue;
+    u32 nbits = 0;
+    if (cudaMemcpy(&nbits, e.scratch + L.scratch_off[i] + br_split_code_end_off(hm[i], ha[i]), 4, cudaMemcpyDeviceToHost) != cudaSuccess)
+      goto done;
+    std::vector<u32> bits((nbits + 31) / 32 + 1);
+    if (cudaMemcpy(bits.data(), e.outbits + L.out_off[i], bits.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+    br_split_record_bits(recs[r++], bits.data(), nbits);
+  }
+  ret = (long)br_split_put(recs, h_out, out_cap);
+done:
+  cudaGetLastError();
+  A.release();
+  return ret;
 }

@@ -75,14 +75,22 @@ double oracle_fast_log2(size_t v) { return fast_log2(v); }
  *       (cur_m + best_len > rmask); srch_ring_skip: a candidate skipped by prev_m + best_len > rmask;
  *   srch_tie_max: a candidate as long as a best length that already equals max_length (the stale byte decides);
  *   srch_wrap_cut: a ring cut short by a wrapped uint16 counter (oracle_search_probe);
- *   srch_dict_hit: a static-dictionary item taken; srch_gate_closed: the dictionary gate (hash.h:186) closed */
+ *   srch_dict_hit: a static-dictionary item taken; srch_gate_closed: the dictionary gate (hash.h:186) closed
+ * And for the greedy block splitter (splitter_finish_block, tests/split_cases.py), counted at every block decision:
+ *   split_tie: a block kept apart from a new type only because a diff equals the threshold exactly (`>` against `>=`);
+ *   back_tie: a block merged, not sent back to the type before last, only because diff[1] == diff[0] - 20 exactly;
+ *   split_clamp: a histogram of cost below 1 bit per symbol, raised to its symbol count (bit_cost.c:35);
+ *   split_pad / split_pad_empty: a final block shorter than the shortest block, padded to it (empty: the symbols
+ *       ended exactly at a block's end); split_grow: a second merge in a row that grows the target block size;
+ *   cmd_cap / dist_cap: compressed metablocks whose command / distance split reached 256 types */
 #define EDGE_FIELDS(X) X(retry_lit) X(retry_cmd) X(retry_dist) X(retry_other) X(retry_cl) X(retry_fast) \
   X(simple_nsym1) X(simple_nsym2) X(simple_nsym3) X(simple_nsym4) X(simple_select0) X(simple_select1) X(rle_lt16) X(rle_lt28) X(rle_full) X(rle_holes) \
   X(reps7) X(reps11) X(rle_use_nz) X(rle_use_z) X(ctx_nc1) X(ctx_nc2) X(ctx_nc3) X(ctx_nc13) X(lit_cap_nc1) \
   X(lit_cap_nc2) X(lit_cap_nc3) X(lit_cap_nc13) X(split_back) X(max_lit_types) X(max_lit_trees) X(max_cmd_types) \
   X(max_dist_types) X(max_insert) X(max_copy) X(max_block_len) X(max_distance) X(codes) \
   X(rle_good) X(rle_stride) X(cl_single) X(cl_skip2) X(cl_skip3) X(cl_trim) \
-  X(srch_dc_len2) X(srch_ring_break) X(srch_ring_skip) X(srch_tie_max) X(srch_wrap_cut) X(srch_dict_hit) X(srch_gate_closed)
+  X(srch_dc_len2) X(srch_ring_break) X(srch_ring_skip) X(srch_tie_max) X(srch_wrap_cut) X(srch_dict_hit) X(srch_gate_closed) \
+  X(split_tie) X(back_tie) X(split_clamp) X(split_pad) X(split_pad_empty) X(split_grow) X(cmd_cap) X(dist_cap)
 #define EDGE_MEMBER(f) uint64_t f;
 #define EDGE_NAME(f) #f ","
 static _Thread_local struct { EDGE_FIELDS(EDGE_MEMBER) } g_edge;   /* per thread: callers may run the oracle in a pool */
@@ -623,8 +631,9 @@ static void create_backward_references(Enc* e, size_t num_bytes, size_t position
 }
 
 /* --------------------------------------------------------- entropy helpers */
-/* bit_cost.c:18 BrotliBitsEntropy -- sequential order, no FMA */
-static double bits_entropy(const uint32_t* pop, size_t size) {
+/* bit_cost.c:18 BrotliBitsEntropy -- sequential order, no FMA; clamps (nullable) counts the histograms raised to their
+   symbol count */
+static double bits_entropy_c(const uint32_t* pop, size_t size, uint64_t* clamps) {
   size_t sum = 0, i;
   double retval = 0;
   for (i = 0; i < size; ++i) {
@@ -633,9 +642,10 @@ static double bits_entropy(const uint32_t* pop, size_t size) {
     retval -= (double)p * fast_log2(p);
   }
   if (sum) retval += (double)sum * fast_log2(sum);
-  if (retval < (double)sum) retval = (double)sum;
+  if (retval < (double)sum) { retval = (double)sum; if (clamps) ++*clamps; }
   return retval;
 }
+static double bits_entropy(const uint32_t* pop, size_t size) { return bits_entropy_c(pop, size, NULL); }
 /* encode.c:258 EstimateEntropy */
 static double estimate_entropy(const uint32_t* pop, size_t size) {
   size_t total = 0, i;
@@ -1044,12 +1054,15 @@ static void splitter_finish_block(Splitter* s, int is_final) {
   double* last_entropy = s->last_entropy;
   uint32_t* H = s->histograms;
   size_t i, k;
-  if (s->block_size < s->min_block_size) s->block_size = s->min_block_size;
+  if (s->block_size < s->min_block_size) {
+    if (s->block_size) ++g_edge.split_pad; else if (s->num_blocks) ++g_edge.split_pad_empty;
+    s->block_size = s->min_block_size;
+  }
   if (s->num_blocks == 0) {
     split->lengths[0] = (uint32_t)s->block_size;
     split->types[0] = 0;
     for (i = 0; i < nc; ++i) {
-      last_entropy[i] = bits_entropy(H + i * A, A);
+      last_entropy[i] = bits_entropy_c(H + i * A, A, &g_edge.split_clamp);
       last_entropy[nc + i] = last_entropy[i];
     }
     ++s->num_blocks; ++split->num_types;
@@ -1060,14 +1073,20 @@ static void splitter_finish_block(Splitter* s, int is_final) {
     double entropy[13], combined_entropy[26], diff[2] = {0.0, 0.0};
     for (i = 0; i < nc; ++i) {
       size_t cur = s->curr_ix + i, j;
-      entropy[i] = bits_entropy(H + cur * A, A);
+      entropy[i] = bits_entropy_c(H + cur * A, A, &g_edge.split_clamp);
       for (j = 0; j < 2; ++j) {
         size_t jx = j * nc + i, last = s->last_ix[j] + i;
         for (k = 0; k < A; ++k) s->combined[jx * A + k] = H[cur * A + k] + H[last * A + k];
-        combined_entropy[jx] = bits_entropy(s->combined + jx * A, A);
+        combined_entropy[jx] = bits_entropy_c(s->combined + jx * A, A, &g_edge.split_clamp);
         diff[j] += combined_entropy[jx] - entropy[i] - last_entropy[jx];
       }
     }
+    if (split->num_types < s->max_block_types && diff[0] >= s->split_threshold && diff[1] >= s->split_threshold &&
+        (diff[0] == s->split_threshold || diff[1] == s->split_threshold))
+      ++g_edge.split_tie;
+    else if (!(split->num_types < s->max_block_types && diff[0] > s->split_threshold && diff[1] > s->split_threshold) &&
+             diff[1] == diff[0] - 20.0)
+      ++g_edge.back_tie;
     if (split->num_types < s->max_block_types &&
         diff[0] > s->split_threshold && diff[1] > s->split_threshold) {
       split->lengths[s->num_blocks] = (uint32_t)s->block_size;
@@ -1102,7 +1121,7 @@ static void splitter_finish_block(Splitter* s, int is_final) {
         memset(H + (s->curr_ix + i) * A, 0, A * 4);
       }
       s->block_size = 0;
-      if (++s->merge_last_count > 1) s->target_block_size += s->min_block_size;
+      if (++s->merge_last_count > 1) { s->target_block_size += s->min_block_size; ++g_edge.split_grow; }
     }
   }
   if (is_final) {
@@ -1377,68 +1396,83 @@ static void store_cmd_extra(const Cmd* c, BitW* w) {
   wbits(w, insn + kCopyExtra[cc], (copyv << insn) | insv);
 }
 
-/* metablock.c:708 BrotliBuildMetaBlockGreedyInternal + :841 OptimizeHistograms
-   + brotli_bit_stream.c:947 BrotliStoreMetaBlock */
-static void store_compressed_metablock(Enc* e, size_t start_pos, size_t length,
-                                       int is_last, BitW* w) {
-  const uint8_t* in = e->data;
-  const Cmd* cmds = e->cmds; const size_t ncmd = e->num_cmds;
-  size_t nctx = 1; const uint32_t* smap = NULL;
+/* A compressed metablock in the making: the literal context choice, the greedy splits with their histograms, then
+   the context map and the block encoders of its header. */
+typedef struct {
+  size_t nctx; const uint32_t* smap;
   Split lit_split, cmd_split, dist_split;
   Splitter ls, cs, ds;
+  uint32_t* lit_cmap; size_t lit_cmap_size;
+  BlockEnc le, ce, de;
+  HTree* tree;
+} MbStore;
+
+/* encode.c:561 DecideOverLiteralContextModeling (skipped under disable_ctx) + metablock.c:708
+   BrotliBuildMetaBlockGreedyInternal: the splits and their histograms, not yet smoothed. */
+static void mb_build_splits(const Enc* e, size_t start_pos, int disable_ctx, size_t length, MbStore* s) {
+  const uint8_t* in = e->data;
+  const Cmd* cmds = e->cmds; const size_t ncmd = e->num_cmds;
   size_t num_literals = 0, i, pos;
   uint8_t p1 = e->prev_byte, p2 = e->prev_byte2;
-  uint32_t* lit_cmap = NULL; size_t lit_cmap_size = 0;
-  HTree* tree = (HTree*)malloc(sizeof(HTree) * (2 * 704 + 1));
-  uint8_t good_for_rle[704];
-  BlockEnc le, ce, de;
-
-  decide_context_modeling(e, start_pos, length, &nctx, &smap);
+  memset(s, 0, sizeof(*s));
+  s->nctx = 1;
+  if (!disable_ctx) decide_context_modeling(e, start_pos, length, &s->nctx, &s->smap);
   for (i = 0; i < ncmd; ++i) num_literals += cmds[i].insert_len;
-  splitter_init(&ls, 256, nctx, 512, 400.0, num_literals, &lit_split);
-  splitter_init(&cs, 704, 1, 1024, 500.0, ncmd, &cmd_split);
-  splitter_init(&ds, 64, 1, 512, 100.0, ncmd, &dist_split);
+  splitter_init(&s->ls, 256, s->nctx, 512, 400.0, num_literals, &s->lit_split);
+  splitter_init(&s->cs, 704, 1, 1024, 500.0, ncmd, &s->cmd_split);
+  splitter_init(&s->ds, 64, 1, 512, 100.0, ncmd, &s->dist_split);
   pos = start_pos;
   for (i = 0; i < ncmd; ++i) {
     const Cmd c = cmds[i]; size_t j;
-    splitter_add(&cs, c.cmd_prefix, 0);
+    splitter_add(&s->cs, c.cmd_prefix, 0);
     for (j = c.insert_len; j != 0; --j) {
       uint8_t lit = in[pos];
-      if (nctx == 1) splitter_add(&ls, lit, 0);
-      else splitter_add(&ls, lit, smap[CTX_UTF8(p1, p2)]);
+      if (s->nctx == 1) splitter_add(&s->ls, lit, 0);
+      else splitter_add(&s->ls, lit, s->smap[CTX_UTF8(p1, p2)]);
       p2 = p1; p1 = lit; ++pos;
     }
     pos += cmd_copy_len(&c);
     if (cmd_copy_len(&c)) {
       p2 = in[pos - 2]; p1 = in[pos - 1];
-      if (c.cmd_prefix >= 128) splitter_add(&ds, c.dist_prefix & 0x3FF, 0);
+      if (c.cmd_prefix >= 128) splitter_add(&s->ds, c.dist_prefix & 0x3FF, 0);
     }
   }
-  splitter_finish_block(&ls, 1);
-  splitter_finish_block(&cs, 1);
-  splitter_finish_block(&ds, 1);
+  splitter_finish_block(&s->ls, 1);
+  splitter_finish_block(&s->cs, 1);
+  splitter_finish_block(&s->ds, 1);
+}
+
+/* metablock.c:677 MapStaticContexts, :841 OptimizeHistograms and brotli_bit_stream.c:947 BrotliStoreMetaBlock up to
+   the last prefix code: the header, the block-split codes, the context maps and every code. */
+static void mb_store_header_and_codes(MbStore* s, size_t length, int is_last, BitW* w) {
+  const size_t nctx = s->nctx;
+  size_t i;
+  uint8_t good_for_rle[704];
+  s->tree = (HTree*)malloc(sizeof(HTree) * (2 * 704 + 1));
   if (nctx > 1) {  /* metablock.c:677 MapStaticContexts */
     size_t j;
-    lit_cmap_size = lit_split.num_types << 6;
-    lit_cmap = (uint32_t*)malloc(lit_cmap_size * 4);
-    for (i = 0; i < lit_split.num_types; ++i)
-      for (j = 0; j < 64; ++j) lit_cmap[(i << 6) + j] = (uint32_t)(i * nctx) + smap[j];
+    s->lit_cmap_size = s->lit_split.num_types << 6;
+    s->lit_cmap = (uint32_t*)malloc(s->lit_cmap_size * 4);
+    for (i = 0; i < s->lit_split.num_types; ++i)
+      for (j = 0; j < 64; ++j) s->lit_cmap[(i << 6) + j] = (uint32_t)(i * nctx) + s->smap[j];
   }
   if (nctx == 1) ++g_edge.ctx_nc1; else if (nctx == 2) ++g_edge.ctx_nc2; else if (nctx == 3) ++g_edge.ctx_nc3; else ++g_edge.ctx_nc13;
-  if (lit_split.num_types == 256 / nctx) {
+  if (s->lit_split.num_types == 256 / nctx) {
     if (nctx == 1) ++g_edge.lit_cap_nc1; else if (nctx == 2) ++g_edge.lit_cap_nc2; else if (nctx == 3) ++g_edge.lit_cap_nc3;
     else ++g_edge.lit_cap_nc13;
   }
-  EDGE_MAX(max_lit_types, lit_split.num_types); EDGE_MAX(max_lit_trees, ls.histograms_size);
-  g_edge.codes += ls.histograms_size + cs.histograms_size + ds.histograms_size;
-  EDGE_MAX(max_cmd_types, cmd_split.num_types); EDGE_MAX(max_dist_types, dist_split.num_types);
-  { const Split* sp[3] = {&lit_split, &cmd_split, &dist_split}; size_t k;   /* lengths are stored with 2+ types only */
+  if (s->cmd_split.num_types == 256) ++g_edge.cmd_cap;
+  if (s->dist_split.num_types == 256) ++g_edge.dist_cap;
+  EDGE_MAX(max_lit_types, s->lit_split.num_types); EDGE_MAX(max_lit_trees, s->ls.histograms_size);
+  g_edge.codes += s->ls.histograms_size + s->cs.histograms_size + s->ds.histograms_size;
+  EDGE_MAX(max_cmd_types, s->cmd_split.num_types); EDGE_MAX(max_dist_types, s->dist_split.num_types);
+  { const Split* sp[3] = {&s->lit_split, &s->cmd_split, &s->dist_split}; size_t k;   /* lengths are stored with 2+ types only */
     for (k = 0; k < 3; ++k)
       if (sp[k]->num_types > 1)
         for (i = 0; i < sp[k]->num_blocks; ++i) EDGE_MAX(max_block_len, sp[k]->lengths[i]); }
-  for (i = 0; i < ls.histograms_size; ++i) optimize_counts_for_rle(256, ls.histograms + i * 256, good_for_rle);
-  for (i = 0; i < cs.histograms_size; ++i) optimize_counts_for_rle(704, cs.histograms + i * 704, good_for_rle);
-  for (i = 0; i < ds.histograms_size; ++i) optimize_counts_for_rle(64, ds.histograms + i * 64, good_for_rle);
+  for (i = 0; i < s->ls.histograms_size; ++i) optimize_counts_for_rle(256, s->ls.histograms + i * 256, good_for_rle);
+  for (i = 0; i < s->cs.histograms_size; ++i) optimize_counts_for_rle(704, s->cs.histograms + i * 704, good_for_rle);
+  for (i = 0; i < s->ds.histograms_size; ++i) optimize_counts_for_rle(64, s->ds.histograms + i * 64, good_for_rle);
 
   /* header: brotli_bit_stream.c:120 */
   wbits(w, 1, (uint64_t)is_last);
@@ -1446,41 +1480,56 @@ static void store_compressed_metablock(Enc* e, size_t start_pos, size_t length,
   store_mlen(length, w);
   if (!is_last) wbits(w, 1, 0);
 
-  block_enc_init(&le, 256, &lit_split);
-  block_enc_init(&ce, 704, &cmd_split);
-  block_enc_init(&de, 64, &dist_split);
-  build_and_store_block_split_code(&le, tree, w);
-  build_and_store_block_split_code(&ce, tree, w);
-  build_and_store_block_split_code(&de, tree, w);
+  block_enc_init(&s->le, 256, &s->lit_split);
+  block_enc_init(&s->ce, 704, &s->cmd_split);
+  block_enc_init(&s->de, 64, &s->dist_split);
+  build_and_store_block_split_code(&s->le, s->tree, w);
+  build_and_store_block_split_code(&s->ce, s->tree, w);
+  build_and_store_block_split_code(&s->de, s->tree, w);
   wbits(w, 2, 0);  /* NPOSTFIX */
   wbits(w, 4, 0);  /* NDIRECT >> NPOSTFIX */
-  for (i = 0; i < lit_split.num_types; ++i) wbits(w, 2, 2);  /* CONTEXT_UTF8 */
-  if (lit_cmap_size == 0) store_trivial_context_map(ls.histograms_size, 6, tree, w);
-  else encode_context_map(lit_cmap, lit_cmap_size, ls.histograms_size, tree, w);
-  store_trivial_context_map(ds.histograms_size, 2, tree, w);
+  for (i = 0; i < s->lit_split.num_types; ++i) wbits(w, 2, 2);  /* CONTEXT_UTF8 */
+  if (s->lit_cmap_size == 0) store_trivial_context_map(s->ls.histograms_size, 6, s->tree, w);
+  else encode_context_map(s->lit_cmap, s->lit_cmap_size, s->ls.histograms_size, s->tree, w);
+  store_trivial_context_map(s->ds.histograms_size, 2, s->tree, w);
 
-  le.depths = (uint8_t*)malloc(ls.histograms_size * 256 + 1); le.bits = (uint16_t*)malloc(ls.histograms_size * 512 + 2);
-  ce.depths = (uint8_t*)malloc(cs.histograms_size * 704 + 1); ce.bits = (uint16_t*)malloc(cs.histograms_size * 1408 + 2);
-  de.depths = (uint8_t*)malloc(ds.histograms_size * 64 + 1); de.bits = (uint16_t*)malloc(ds.histograms_size * 128 + 2);
-  for (i = 0; i < ls.histograms_size; ++i)
-    build_and_store_tree(ls.histograms + i * 256, 256, 256, tree, le.depths + i * 256, le.bits + i * 256, w);
-  for (i = 0; i < cs.histograms_size; ++i)
-    build_and_store_tree(cs.histograms + i * 704, 704, 704, tree, ce.depths + i * 704, ce.bits + i * 704, w);
-  for (i = 0; i < ds.histograms_size; ++i)
-    build_and_store_tree(ds.histograms + i * 64, 64, 64, tree, de.depths + i * 64, de.bits + i * 64, w);
+  s->le.depths = (uint8_t*)malloc(s->ls.histograms_size * 256 + 1); s->le.bits = (uint16_t*)malloc(s->ls.histograms_size * 512 + 2);
+  s->ce.depths = (uint8_t*)malloc(s->cs.histograms_size * 704 + 1); s->ce.bits = (uint16_t*)malloc(s->cs.histograms_size * 1408 + 2);
+  s->de.depths = (uint8_t*)malloc(s->ds.histograms_size * 64 + 1); s->de.bits = (uint16_t*)malloc(s->ds.histograms_size * 128 + 2);
+  for (i = 0; i < s->ls.histograms_size; ++i)
+    build_and_store_tree(s->ls.histograms + i * 256, 256, 256, s->tree, s->le.depths + i * 256, s->le.bits + i * 256, w);
+  for (i = 0; i < s->cs.histograms_size; ++i)
+    build_and_store_tree(s->cs.histograms + i * 704, 704, 704, s->tree, s->ce.depths + i * 704, s->ce.bits + i * 704, w);
+  for (i = 0; i < s->ds.histograms_size; ++i)
+    build_and_store_tree(s->ds.histograms + i * 64, 64, 64, s->tree, s->de.depths + i * 64, s->de.bits + i * 64, w);
+}
+static void mb_free(MbStore* s) {
+  free(s->le.depths); free(s->le.bits); free(s->ce.depths); free(s->ce.bits); free(s->de.depths); free(s->de.bits);
+  free(s->lit_cmap); free(s->tree);
+  splitter_free(&s->ls); splitter_free(&s->cs); splitter_free(&s->ds);
+}
 
+static void store_compressed_metablock(Enc* e, size_t start_pos, size_t length,
+                                       int is_last, BitW* w) {
+  const uint8_t* in = e->data;
+  const Cmd* cmds = e->cmds; const size_t ncmd = e->num_cmds;
+  size_t i, pos;
+  uint8_t p1, p2;
+  MbStore s;
+  mb_build_splits(e, start_pos, 0, length, &s);
+  mb_store_header_and_codes(&s, length, is_last, w);
   pos = start_pos; p1 = e->prev_byte; p2 = e->prev_byte2;
   for (i = 0; i < ncmd; ++i) {
     const Cmd c = cmds[i]; size_t j;
     edge_cmd(&c, e->lgwin);
-    store_symbol(&ce, c.cmd_prefix, w);
+    store_symbol(&s.ce, c.cmd_prefix, w);
     store_cmd_extra(&c, w);
-    if (lit_cmap_size == 0) {
-      for (j = c.insert_len; j != 0; --j) { store_symbol(&le, in[pos], w); ++pos; }
+    if (s.lit_cmap_size == 0) {
+      for (j = c.insert_len; j != 0; --j) { store_symbol(&s.le, in[pos], w); ++pos; }
     } else {
       for (j = c.insert_len; j != 0; --j) {
         uint8_t lit = in[pos];
-        store_symbol_ctx(&le, lit, CTX_UTF8(p1, p2), lit_cmap, w);
+        store_symbol_ctx(&s.le, lit, CTX_UTF8(p1, p2), s.lit_cmap, w);
         p2 = p1; p1 = lit; ++pos;
       }
     }
@@ -1488,16 +1537,81 @@ static void store_compressed_metablock(Enc* e, size_t start_pos, size_t length,
     if (cmd_copy_len(&c)) {
       p2 = in[pos - 2]; p1 = in[pos - 1];
       if (c.cmd_prefix >= 128) {
-        store_symbol(&de, c.dist_prefix & 0x3FF, w);
+        store_symbol(&s.de, c.dist_prefix & 0x3FF, w);
         wbits(w, c.dist_prefix >> 10, c.dist_extra);
       }
     }
   }
   if (is_last) { w->ix = (w->ix + 7u) & ~(size_t)7u; w->buf[w->ix >> 3] = 0; }
-  free(le.depths); free(le.bits); free(ce.depths); free(ce.bits); free(de.depths); free(de.bits);
-  free(lit_cmap); free(tree);
-  splitter_free(&ls); splitter_free(&cs); splitter_free(&ds);
+  mb_free(&s);
 }
+
+/* The entropy stage of quality 4..9 up to the last prefix code, on metablocks the caller describes (the counterpart of
+   the product's br_debug_split hook, with its arguments): mbw holds 7 words per metablock (start, end, first command,
+   command count, is_last, compress, base: the first byte of its stream, where the literal context starts from zeros).
+   cmds: 16 bytes each (oracle_make_cmd), covering the input in order.  For every compressed metablock the record of
+   br_split_record: which, num_types[3], num_blocks[3], the bit count; per category types and lengths (a word each); the
+   histograms before smoothing (literal rows of 256, command rows of 704, distance rows of 64); then the header, the
+   block-split codes, the context maps and every prefix code as (bits + 31) / 32 words.  Writes at most cap words to
+   out and returns the words the records take, 0 on a description that does not hold together (metablocks that do not
+   follow each other, or commands that do not cover their metablock exactly), as br_split_synth rejects it. */
+size_t oracle_split(const uint8_t* in, size_t n, const Cmd* cmds, size_t ncmd, const uint32_t* mbw, size_t n_mbs,
+                    int quality, size_t size_hint, int disable_ctx, uint32_t* out, size_t cap) {
+  size_t k = 0, m, c = 0, i, covered = 0;
+#define PUT(v) do { if (k < cap) out[k] = (uint32_t)(v); ++k; } while (0)
+  if (quality < 4 || quality > 9) return 0;
+  for (m = 0; m < n_mbs; ++m) {
+    const uint32_t* w = mbw + 7 * m;
+    const size_t start = w[0], end = w[1], base = w[6];
+    Enc e; MbStore s; BitW bw; uint8_t* buf; size_t cat;
+    if (w[2] != c || w[3] == 0 || c + w[3] > ncmd || end <= start || end > n || base > start || start != covered) return 0;
+    { size_t span = 0;
+      for (i = c; i < c + w[3]; ++i) span += (size_t)cmds[i].insert_len + cmd_copy_len(&cmds[i]);
+      if (span != end - start) return 0; }
+    c += w[3]; covered = end;
+    if (!w[5]) continue;
+    memset(&e, 0, sizeof(e));
+    e.quality = quality; e.size_hint = size_hint; e.data = in; e.n = n;
+    e.cmds = (Cmd*)(cmds + w[2]); e.num_cmds = w[3];
+    e.prev_byte = start >= base + 1 ? in[start - 1] : 0; e.prev_byte2 = start >= base + 2 ? in[start - 2] : 0;
+    mb_build_splits(&e, start, disable_ctx, end - start, &s);
+    PUT(s.nctx);
+    PUT(s.lit_split.num_types); PUT(s.cmd_split.num_types); PUT(s.dist_split.num_types);
+    PUT(s.lit_split.num_blocks); PUT(s.cmd_split.num_blocks); PUT(s.dist_split.num_blocks);
+    { const size_t at_bits = k; const Split* sp[3] = {&s.lit_split, &s.cmd_split, &s.dist_split};
+      const Splitter* sr[3] = {&s.ls, &s.cs, &s.ds};
+      PUT(0);
+      for (cat = 0; cat < 3; ++cat) {
+        for (i = 0; i < sp[cat]->num_blocks; ++i) PUT(sp[cat]->types[i]);
+        for (i = 0; i < sp[cat]->num_blocks; ++i) PUT(sp[cat]->lengths[i]);
+      }
+      for (cat = 0; cat < 3; ++cat)
+        for (i = 0; i < sr[cat]->histograms_size * sr[cat]->alphabet; ++i) PUT(sr[cat]->histograms[i]);
+      buf = (uint8_t*)calloc(2 * (end - start) + 4096 + 1024 * (s.ls.histograms_size + s.cs.histograms_size + s.ds.histograms_size), 1);
+      bw.buf = buf; bw.ix = 0;
+      mb_store_header_and_codes(&s, end - start, (int)w[4], &bw);
+      if (at_bits < cap) out[at_bits] = (uint32_t)bw.ix;
+      for (i = 0; i < (bw.ix + 31) / 32; ++i) { uint32_t v; memcpy(&v, buf + 4 * i, 4); PUT(v); }
+      free(buf); }
+    mb_free(&s);
+  }
+#undef PUT
+  return c == ncmd && covered == n ? k : 0;
+}
+/* The static literal context map of nctx contexts (2, 3 or 13; encode.c:277, :341), 64 entries. */
+int oracle_static_context_map(size_t nctx, uint32_t* out) {
+  const uint32_t* map = nctx == 2 ? kCtxMapSimpleUTF8 : nctx == 3 ? kCtxMapContinuation : nctx == 13 ? kCtxMapComplexUTF8 : NULL;
+  if (!map) return 0;
+  memcpy(out, map, 64 * 4);
+  return 1;
+}
+/* command.h:120 InitCommand for callers that build command lists (the split tests): insert, copy length, the delta of
+   the copy length code and the distance code (0..15: the last-distance codes, else distance + 15). */
+void oracle_make_cmd(uint32_t insert, uint32_t copy, int copy_code_delta, uint32_t dcode, Cmd* out) {
+  init_cmd(out, insert, copy, copy_code_delta, dcode);
+}
+/* command.h:138 InitInsertCommand */
+void oracle_make_insert_cmd(uint32_t insert, Cmd* out) { init_insert_cmd(out, insert); }
 
 static void emit(Enc* e, const uint8_t* p, size_t n) {
   if (e->out_pos + n > e->out_cap) { e->overflow = 1; return; }

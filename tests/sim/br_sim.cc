@@ -397,6 +397,18 @@ struct SimEnt {
   std::vector<u8> scratch;
   BrMbLayout L;
 };
+// k_mb_setup and (qualities 4..9) k_split for one metablock, with a one-thread CTA
+static void sim_split_mb(const BrStream& s, const BrEnt& e, const BrMetaBlock& mb, BrMbAux& a, u8* sc, u32* smem) {
+  BrMbMem* M = (BrMbMem*)sc;
+  br_mb_aux_init(a, mb, e, s.P.disable_ctx ? 1u : br_decide_context_modeling(s, mb.start, mb.end - mb.start, M->sc.rle_syms));
+  if (s.P.mb_kind) return;
+  for (int cat = 0; cat < 3; ++cat) {
+    const BrSplitCat k = br_split_cat(cat, a.which);
+    const u32 nblk = br_mb2_nblk(cat, mb.nlit, mb.ncmd);
+    br_split_cta(s, e, mb, a, cat, k.A, k.nc, k.min_block, k.thr, a.nsym[cat], br_mb2_types(sc, a, cat, nblk),
+                 br_mb2_lengths(sc, a, cat, nblk), BR_SPLIT_HIST(M, cat), smem);
+  }
+}
 static void sim_entropy2(SimStream& m, SimEnt& E) {
   BrStream& s = m.s;
   u32 nm = s.counters[1], C = s.counters[2];
@@ -427,21 +439,8 @@ static void sim_entropy2(SimStream& m, SimEnt& E) {
     if (!mb.compress) continue;
     BrMbAux& a = E.aux[i];
     u8* sc = E.scratch.data() + E.L.scratch_off[i];
-    BrMbMem* M = (BrMbMem*)sc;
-    a.which = s.P.disable_ctx ? 1u : br_decide_context_modeling(s, mb.start, mb.end - mb.start, M->sc.rle_syms);
-    a.lit_base = E.lit_ord[mb.cmd_off]; a.dist_base = E.dist_ord[mb.cmd_off];
-    a.nsym[0] = mb.nlit; a.nsym[1] = mb.ncmd; a.nsym[2] = E.dist_ord[mb.cmd_off + mb.ncmd] - a.dist_base;
-    u32 off = br_align8((u32)sizeof(BrMbMem));
-    for (int cat = 0; cat < 3; ++cat) { a.var_off[cat] = off; off += br_mb2_var_bytes(br_mb2_nblk(cat, mb.nlit, mb.ncmd)); }
+    sim_split_mb(s, e, mb, a, sc, smem.data());
     if (s.P.mb_kind) { br_prep_flat(s, e, mb, a, sc, E.outbits.data() + E.L.out_off[i]); continue; }
-    const u32 A[3] = {256, 704, 64}, NC[3] = {a.which, 1, 1}, MB[3] = {512, 1024, 512};
-    const double TH[3] = {400.0, 500.0, 100.0};
-    u32* H[3] = {M->lit_H, M->cmd_H, M->dist_H};
-    for (int cat = 0; cat < 3; ++cat) {
-      u32 nblk = br_mb2_nblk(cat, mb.nlit, mb.ncmd);
-      br_split_cta(s, e, mb, a, cat, A[cat], NC[cat], MB[cat], TH[cat], a.nsym[cat], br_mb2_types(sc, a, cat, nblk),
-                   br_mb2_lengths(sc, a, cat, nblk), H[cat], smem.data());
-    }
     br_prep_codes(s, mb, a, sc, E.outbits.data() + E.L.out_off[i]);
   }
   for (u32 o = 0; o < e.total_lits; ++o) br_lit_bits(s, e, o);
@@ -576,6 +575,53 @@ extern "C" int sim_debug_codes(u32 n_mbs, const u32* counts, const u32* histos, 
   }
   info[0] = total; info[1] = warps ? 1u : 2u; info[2] = nwk;
   return 1;
+}
+
+// E0..E4 on metablocks the caller describes: the counterpart of the product's br_debug_split hook, with its arguments.  E2
+// and E3 by sim_split_mb (one-thread CTAs), E4 by br_prep_codes, metablock by metablock, on a scratch that starts with
+// the device hook's pattern.
+extern "C" long sim_debug_split(const u8* in, u32 n, const BrCmd* cmds, u32 ncmd, const u32* mbw, u32 n_mbs, int quality,
+                                u32 size_hint, int disable_ctx, u32* out, size_t out_cap) {
+  if (n == 0 || n_mbs == 0 || quality < 4 || quality > 9) return 0;
+  BrStream s; memset(&s, 0, sizeof(s));
+  s.P.quality = quality; s.P.n = n; s.P.size_hint = size_hint; s.P.disable_ctx = disable_ctx ? 1u : 0u;
+  std::vector<BrMetaBlock> mbs; BrMbLayout L;
+  if (!br_split_synth(s.P, mbw, n_mbs, cmds, ncmd, mbs, L)) return 0;
+  std::vector<u8> data((size_t)n + 64, 0);
+  memcpy(data.data(), in, n);
+  s.data = data.data(); s.mbs = mbs.data();
+  br_bind_tables(s, g_t.blob.data(), g_t.log2tab.data(), (u32)g_t.log2tab.size());
+  BrEnt e; memset(&e, 0, sizeof(e));
+  std::vector<u32> lit_ord(ncmd + 1, 0), cmd_pos(ncmd + 1, 0), dist_ord(ncmd + 1, 0);
+  for (u32 i = 0; i < ncmd; ++i) {
+    u32 a, b, d; br_cmd_scan_inputs(cmds[i], &a, &b, &d);
+    lit_ord[i + 1] = lit_ord[i] + a; cmd_pos[i + 1] = cmd_pos[i] + b; dist_ord[i + 1] = dist_ord[i] + d;
+  }
+  std::vector<u32> lit_pos(lit_ord[ncmd] + 1), lit_cmd(lit_ord[ncmd] + 1), outbits(L.out_words + 64, 0);
+  std::vector<u16> dist_sym(dist_ord[ncmd] + 1);
+  std::vector<BrMbAux> aux(n_mbs);
+  std::vector<u8> sc(L.scratch_bytes + 256, 0xA5);
+  e.cmds = cmds; e.total_cmds = ncmd; e.total_lits = lit_ord[ncmd]; e.total_dist = dist_ord[ncmd];
+  e.lit_ord = lit_ord.data(); e.cmd_pos = cmd_pos.data(); e.dist_ord = dist_ord.data();
+  e.lit_pos = lit_pos.data(); e.lit_cmd = lit_cmd.data(); e.dist_sym = dist_sym.data();
+  e.aux = aux.data(); e.scratch = sc.data(); e.scratch_off = L.scratch_off.data();
+  e.outbits = outbits.data(); e.out_off = L.out_off.data();
+  for (u32 c = 0; c < ncmd; c += BR_WARP) br_expand_cmds(e, c);
+  std::vector<u32> smem(64 * 1024);
+  std::vector<std::vector<u32>> recs;
+  for (u32 i = 0; i < n_mbs; ++i) {
+    if (!mbs[i].compress) continue;
+    u8* msc = sc.data() + L.scratch_off[i];
+    sim_split_mb(s, e, mbs[i], aux[i], msc, smem.data());
+    recs.emplace_back();
+    br_split_record(mbs[i], aux[i], msc, recs.back());
+    u32* mout = outbits.data() + L.out_off[i];
+    br_prep_codes(s, mbs[i], aux[i], msc, mout);
+    u32 nbits;
+    memcpy(&nbits, msc + br_split_code_end_off(mbs[i], aux[i]), 4);
+    br_split_record_bits(recs.back(), mout, nbits);
+  }
+  return (long)br_split_put(recs, out, out_cap);
 }
 #endif
 
