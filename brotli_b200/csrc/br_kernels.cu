@@ -289,16 +289,17 @@ __global__ void k_snapshot_update(BrStream s, u32* __restrict__ storedS, u32* __
 }
 
 // ---------------------------------------------------------------------------- warp-task kernels
-// k_walk<G, M>: G and M as br_walk_dispatch (br_params.h) picks them
+// k_walk<F, M>: the walker form F and M as br_walk_dispatch (br_params.h) picks them; BR_WALK_WARPS warps per block
 #ifndef BR_WALK1_MINB
 #define BR_WALK1_MINB 8
 #endif
-template <int G, bool M>
-__global__ void __launch_bounds__(128, G <= 2 ? BR_WALK1_MINB : G == 4 ? 5 : 4) k_walk(BrStream s) {
+template <int F, bool M>
+__global__ void __launch_bounds__(32 * BR_WALK_WARPS, BR_FORM_G(F) <= 2 ? BR_WALK1_MINB : BR_FORM_G(F) == 4 ? 5 : 4)
+k_walk(BrStream s) {
   u32 t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (t >= s.counters[5]) return;
   const u32 b = br_sched_entry(s, t);
-  br_walk_block<G, M>(s, b, s.forced && b == s.counters[6]);
+  br_walk_block<F, M>(s, b, s.forced && b == s.counters[6]);
 }
 // positions covered by the runs of this launch (br_chain.h br_cover_run); before k_commit
 __global__ void k_cover(BrStream s) {
@@ -787,8 +788,8 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
       CK(cudaMemsetAsync(s.counters + 4, 0, 4, st));
       CK(cudaMemsetAsync(s.counters + 16, 0, 4, st));
       cudaEventRecord(ev[6], st);
-      const u32 wg = (n_sched + 3) / 4;
-      br_walk_dispatch(P, [&](auto g, auto m) { k_walk<decltype(g)::value, decltype(m)::value><<<wg, 128, 0, st>>>(s); });
+      const u32 wg = (n_sched + BR_WALK_WARPS - 1) / BR_WALK_WARPS;
+      br_walk_dispatch(P, [&](auto g, auto m) { k_walk<decltype(g)::value, decltype(m)::value><<<wg, 32 * BR_WALK_WARPS, 0, st>>>(s); });
       cudaEventRecord(ev[7], st);
       walk_pending = true; ++job->stats.walk_launches; job->stats.launches += 6;
       job->stats.walk_bytes += (u64)n_sched * ch;
@@ -986,10 +987,10 @@ extern "C" __attribute__((visibility("default"))) int br_debug_sort(int quality,
 // Test hook (tests/test_search_probe.py): one match search per probe (br_probe.h), one warp each, from a state the caller
 // specifies.  The index (br_build_index), tagS (k_tags), the S-ordered snapshot (k_build_storedS and its prefix) and, at
 // qualities 2..4, the slot entry points (k_slot_pred) are built by the pipeline's own kernels.
-template <int G>
+template <int F>
 __global__ void k_search_probe(BrStream s, u32* own, const u32* probes, u32 np, u32* res) {
   const u32 t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (t < np) br_probe_search<G>(s, own, probes + (size_t)t * BR_PROBE_WORDS, res + (size_t)t * BR_PROBE_WORDS);
+  if (t < np) br_probe_search<F>(s, own, probes + (size_t)t * BR_PROBE_WORDS, res + (size_t)t * BR_PROBE_WORDS);
 }
 // bounds[0 .. nstreams): the end of every stream of a batch laid end to end (bounds[nstreams - 1] == n; nstreams == 1: one
 // stream).  snap / own: the two stored-bit bitmaps, (n + 31) / 32 words each.  heavy_min: 0 keeps the pipeline's value.

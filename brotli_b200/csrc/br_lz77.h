@@ -98,7 +98,9 @@ struct BrWalk {
   u32 p0, pend;    // p0: first position this walker owns; pend: end of the reference input block
   u32 base;        // first byte of the stream (BrBlockIn::base): ring-buffer positions and distance limits count from it
   int dc[4];       // distance cache; entries 4..15 of the reference (hash.h:80) are derived on the fly
-  u64 dict_l, dict_m;
+  // the static-dictionary counters dict_num_lookups / dict_num_matches (hash.h:49) are dict0 + dl / dict0 + dm: dict0 points
+  // at their values where the walk starts (lo, hi, lo, hi as in BrBlockIn), so that no 64-bit copy rides in registers
+  const u32* dict0;
   u32 dl, dm, gate_checks, gate_fail;
   u32 min_wrap;
   u32 stale;       // the byte the reference finds just past the block end (see oracle)
@@ -194,6 +196,11 @@ BR_DEV u32 br_countS_upto(const BrStream& s, u32 x) {
   return base + acc;
 }
 
+// hash.h:186: the dictionary is searched only while dict_num_matches >= dict_num_lookups >> 7
+BR_DEV bool br_dict_gate_closed(const BrWalk& w) {
+  const u64 l = (((u64)w.dict0[1] << 32) | w.dict0[0]) + w.dl, m = (((u64)w.dict0[3] << 32) | w.dict0[2]) + w.dm;
+  return m < (l >> 7);
+}
 // hash.h:140 TestStaticDictionaryItem
 BR_DEV int br_test_dict_item(const BrWalk& w, u32 len, u32 word_idx, u32 cur, u32 max_length,
                              u32 max_backward, BrSR& out) {
@@ -220,14 +227,14 @@ BR_DEV void br_search_static_dict(BrWalk& w, u32 cur, u32 max_length, u32 max_ba
   const BrStream& s = *w.s;
   BR_W(7, 1);
   ++w.gate_checks;
-  if (w.dict_m < (w.dict_l >> 7)) { ++w.gate_fail; return; }
+  if (br_dict_gate_closed(w)) { ++w.gate_fail; return; }
   u32 key = ((br_ld32u(w.d, cur) * 0x1E35A7BDu) >> (32 - 14)) << 1;
   for (int i = 0; i < 2; ++i, ++key) {
-    ++w.dict_l; ++w.dl;
+    ++w.dl;
     u32 len = br_ldg(s.dict_hash_lengths + key);
     if (len != 0) {
       if (br_test_dict_item(w, len, br_ldg(s.dict_hash_words + key), cur, max_length, max_backward, out)) {
-        ++w.dict_m; ++w.dm;
+        ++w.dm;
       }
     }
   }
@@ -325,9 +332,14 @@ BR_DEV u32 br_next_search(u32 x, u32 apply_rh, u32 window) {
 // candidates leaves 28 of 32 lanes idle.  So at quality 5 the first pass runs over 32 candidate slots
 // [distance cache ++ the newest 28 entries of the ring] -- the reference's order (hash.h:80 first, then the ring newest
 // first) -- with one match-length computation and one fold; further ring rows (32 entries each) follow from j - 28.
-template <int G>
+//
+// F = the walker form (br_walk_form): G, and the ring size where it is fixed at compile time.  Quality 5's form (16
+// entries) compiles the shared pass alone, with the four distance-cache probes as a constant; the forms that read
+// block_bits at run time hold every path.
+template <int F>
 BR_DEV void br_find_longest_match(BrWalk& w, u32 cur, u32 max_length, u32 max_backward,
                                   u32 dict_distance, BrSR& out, BrLook look = {~0u, 0u, 0u}) {
+  constexpr int G = BR_FORM_G(F), RB = BR_FORM_RB(F);
   const BrStream& s = *w.s;
   const BrParams& P = s.P;
   const u8* d = w.d;
@@ -351,7 +363,8 @@ BR_DEV void br_find_longest_match(BrWalk& w, u32 cur, u32 max_length, u32 max_ba
   const u32 key = br_hash_key_v(P, c0);
   const u32 lo = br_ldg(s.seg + key), hi = br_ldg(s.seg + key + 1);
   const u32 j = br_ldg(s.rank + cur);
-  const u32 block_size = 1u << P.block_bits;
+  const u32 block_size = RB ? 1u << RB : 1u << P.block_bits;
+  const u32 ndist = RB ? 4u : P.ndist;   // (qualities 5-6 probe the four last distances: br_derive_params)
   u32 V = block_size;   // ring entries the reference holds (fewer only in a heavy bucket whose counter wrapped)
   u32 collected = 0, jj = j;   // stored ring entries seen so far; the ring's slice of S still to read is [lo, jj)
   bool done = false;           // the ring ends (window, stream start, ring-buffer stop)
@@ -491,7 +504,7 @@ BR_DEV void br_find_longest_match(BrWalk& w, u32 cur, u32 max_length, u32 max_ba
         int mag = (int)((0xE79u >> (2 * ((k - 4) >> 1))) & 3u);
         back_i = (k < 10 ? w.dc[0] : w.dc[1]) + ((k & 1) ? mag : -mag);
       }
-      dvalid[i] = (k < P.ndist) && back_i > 0 && (u32)back_i <= max_backward;
+      dvalid[i] = ((u32)k < ndist) && back_i > 0 && (u32)back_i <= max_backward;
       dback[i] = (u32)back_i;
       da0[i] = dvalid[i] ? br_ld64u(d, cur - (u32)back_i) : 0;
     }
@@ -506,7 +519,7 @@ BR_DEV void br_find_longest_match(BrWalk& w, u32 cur, u32 max_length, u32 max_ba
     bool brk = false;
 #pragma unroll
     for (int i = 0; i < ND; ++i) {
-      if (i * BR_WARP >= P.ndist || brk) break;
+      if ((u32)(i * BR_WARP) >= ndist || brk) break;
       const int k = i * BR_WARP + lane;
       const bool valid = dvalid[i];
       const u32 back = dback[i];
@@ -652,12 +665,12 @@ BR_DEV void br_search_static_dict_shallow(BrWalk& w, u32 cur, u32 max_length, u3
   const BrStream& s = *w.s;
   BR_W(7, 1);
   ++w.gate_checks;
-  if (w.dict_m < (w.dict_l >> 7)) { ++w.gate_fail; return; }
+  if (br_dict_gate_closed(w)) { ++w.gate_fail; return; }
   const u32 key = ((br_ld32u(w.d, cur) * 0x1E35A7BDu) >> (32 - 14)) << 1;
-  ++w.dict_l; ++w.dl;
+  ++w.dl;
   const u32 len = br_ldg(s.dict_hash_lengths + key);
   if (len != 0) {
-    if (br_test_dict_item(w, len, br_ldg(s.dict_hash_words + key), cur, max_length, max_backward, out)) { ++w.dict_m; ++w.dm; }
+    if (br_test_dict_item(w, len, br_ldg(s.dict_hash_words + key), cur, max_length, max_backward, out)) ++w.dm;
   }
 }
 // First index of slot `slot`'s segment of S whose position is >= p (p itself is not in that segment): where a search at p
@@ -827,16 +840,26 @@ BR_DEV u32 br_compute_distance_code(u32 distance, u32 max_distance, const int* d
 // `head` is the first chunk of the sweep this run belongs to (== b when the walker starts here), `sweep_p0` the
 // first position the sweep owns (0xffffffff on entry for the head, which sets it): a walker that continues into the
 // chunks behind its own keeps writing the head's bitmap and reads its own fresh bits from sweep_p0 on.
-// M: the job is a batch of streams (BrParams::multi); with M = false the stream base is the constant 0 and folds away.
-template <int G, bool M = false>
-BR_DEV void br_walk_one(const BrStream& s, u32 b, const BrBlockIn& in, BrBlockOut& o, u32 head, u32& sweep_p0) {
+// F: the walker form (br_walk_form).  M: the job is a batch of streams (BrParams::multi); with M = false the stream base
+// is the constant 0 and folds away.
+// The chunk records -- `in`, `o` and `used` (the state this run really starts from, refined by the warm-up; the caller's
+// `used_rec`, else a local) -- are read and written before and after the per-position loop and at the warm-up crossing
+// only.  The loop carries the parse state alone (position, pending literals, the random-heuristics mark, the distance
+// cache, the counts, the gathered bit word) and one precomputed bound: on the GPU the records sit in the warp's shared
+// memory (br_walk_block), so that none of them holds registers across the search, which needs every register there is
+// at 8 blocks of 4 warps per SM (quality 5).
+template <int F, bool M = false>
+BR_DEV void br_walk_one(const BrStream& s, u32 b, const BrBlockIn& in, BrBlockOut& o, u32 head, u32& sweep_p0,
+                        BrBlockIn* used_rec = nullptr) {
+  constexpr int G = BR_FORM_G(F);
   const BrParams& P = s.P;
   const int lane = br_lane();
+  BrBlockIn used_local;
+  BrBlockIn& used = used_rec ? *used_rec : used_local;
   BrWalk w;
   w.s = &s; w.d = s.data; w.p0 = head == b ? in.start_pos : sweep_p0; w.pend = in.blk_end;
   w.own = s.bits_cur + (size_t)(head & 1u) * s.bits_words;
-  w.dict_l = ((u64)in.dict_l_hi << 32) | in.dict_l_lo;
-  w.dict_m = ((u64)in.dict_m_hi << 32) | in.dict_m_lo;
+  w.dict0 = &in.dict_l_lo;
   w.dl = w.dm = w.gate_checks = w.gate_fail = 0;
   w.min_wrap = 0xffffffffu;
   w.fence_due = false;
@@ -853,9 +876,10 @@ BR_DEV void br_walk_one(const BrStream& s, u32 b, const BrBlockIn& in, BrBlockOu
   u32 position = in.start_pos;
   u32 ext = 0;
   u32 apply_random_heuristics = in.apply_rh;
-  BrBlockIn used = in;     // the state this run really starts from (refined by the warm-up)
+  used = in;
   used.warm = 0;
   w.warming = false;
+  u32 cross_at = 0xffffffffu;   // warm-up: where the parse crosses into the chunk
   if (in.warm && !in.first && in.pos >= in.blk_start + in.warm) {
     // State refinement: parse the last `warm` bytes before the chunk from a neutral state; by the
     // time the parse crosses into the chunk it has usually synchronised with the true parse.
@@ -863,8 +887,8 @@ BR_DEV void br_walk_one(const BrStream& s, u32 b, const BrBlockIn& in, BrBlockOu
     position = in.pos - in.warm;
     w.p0 = 0xffffffffu;
     apply_random_heuristics = position + P.spree;
+    cross_at = in.pos;
   }
-  const u64 dict_l0 = w.dict_l, dict_m0 = w.dict_m;
   const u32 window = P.spree;
   u32 store_end;
   if (in.first) {
@@ -883,6 +907,7 @@ BR_DEV void br_walk_one(const BrStream& s, u32 b, const BrBlockIn& in, BrBlockOu
     }
     apply_random_heuristics = position + window;
   }
+  o.ext_len = ext;
   if (in.first) {
     u32 bytes = pos_end - position;   // what CreateBackwardReferences receives after the extension
     store_end = bytes >= P.htl ? pos_end - P.htl + 1 : position;
@@ -894,18 +919,22 @@ BR_DEV void br_walk_one(const BrStream& s, u32 b, const BrBlockIn& in, BrBlockOu
   // counts from zero and the chain / compaction add the true carry (BrStream::lil_in).
   u32 insert_length = 0;
   u32 ncmd = 0, nlit = 0;
+  // the warm-up's crossing into the chunk: from here on this is the chunk's own run
+  auto cross = [&]() {
+    w.warming = false; w.p0 = position;
+    used.start_pos = position; used.apply_rh = apply_random_heuristics;
+    for (int i = 0; i < 4; ++i) used.dc[i] = w.dc[i];
+    insert_length = 0; ncmd = 0; nlit = 0;
+    w.dl = w.dm = w.gate_checks = w.gate_fail = 0;
+    w.min_wrap = 0xffffffffu;
+  };
+  // The parse goes on while position + htl < pos_end and, but in the block's last chunk, position < in.end: one bound.
+  // (So a crossing always lies inside the chunk proper: the warm-up ends inside the loop or, jumping over it, behind it.)
+  u32 bound = pos_end > P.htl ? pos_end - P.htl : 0u;
+  if (!in.last && in.end < bound) bound = in.end;
   BrCmd* cmds = s.cmd_blocks + (size_t)b * s.cmd_stride;
-  while (position + P.htl < pos_end && (in.last || position < in.end)) {
-    if (w.warming && position >= in.pos) {
-      // crossing: from here on this is the chunk's own run
-      w.warming = false; w.p0 = position;
-      used.start_pos = position; used.apply_rh = apply_random_heuristics;
-      for (int i = 0; i < 4; ++i) used.dc[i] = w.dc[i];
-      insert_length = 0; ncmd = 0; nlit = 0;
-      w.dict_l = dict_l0; w.dict_m = dict_m0; w.dl = w.dm = w.gate_checks = w.gate_fail = 0;
-      w.min_wrap = 0xffffffffu;
-      if (position >= in.end && !in.last) break;
-    }
+  while (position < bound) {
+    if (position >= cross_at) { cross(); cross_at = 0xffffffffu; }
     // One search call site for the primary search and the (up to 4) lazy ones at position + 1
     // (backward_references_inc.h:58-101): the walker's code is dominated by the inlined search.
     u32 max_length = pos_end - position;
@@ -938,7 +967,7 @@ BR_DEV void br_walk_one(const BrStream& s, u32 b, const BrBlockIn& in, BrBlockOu
           }
         }
 #endif
-        br_find_longest_match<G>(w, sp, max_length, md, dd, cur, look);
+        br_find_longest_match<F>(w, sp, max_length, md, dd, cur, look);
       }
       if (!have) {
         sr = cur;
@@ -991,14 +1020,7 @@ BR_DEV void br_walk_one(const BrStream& s, u32 b, const BrBlockIn& in, BrBlockOu
       }
     }
   }
-  if (w.warming) {   // the warm-up parse jumped over the whole chunk (or the block ended)
-    w.warming = false; w.p0 = position;
-    used.start_pos = position; used.apply_rh = apply_random_heuristics;
-    for (int i = 0; i < 4; ++i) used.dc[i] = w.dc[i];
-    insert_length = 0; ncmd = 0; nlit = 0;
-    w.dict_l = dict_l0; w.dict_m = dict_m0; w.dl = w.dm = w.gate_checks = w.gate_fail = 0;
-    w.min_wrap = 0xffffffffu;
-  }
+  if (w.warming) cross();   // the warm-up parse jumped over the whole chunk (or the block ended)
   br_own_flush(w);
   br_own_sync(w);   // a sweep's next chunk starts with a fresh BrWalk: nothing may stay pending
   if (in.last) {
@@ -1009,7 +1031,7 @@ BR_DEV void br_walk_one(const BrStream& s, u32 b, const BrBlockIn& in, BrBlockOu
     o.ncmd = ncmd; o.nlit = nlit; o.out_pos = position; o.last_insert_len = insert_length;
     for (int i = 0; i < 4; ++i) o.dc[i] = w.dc[i];
     o.apply_rh = apply_random_heuristics; o.store_end = store_end;
-    o.ext_len = ext; o.dl = w.dl; o.dm = w.dm;
+    o.dl = w.dl; o.dm = w.dm;
     o.gate_checks = w.gate_checks; o.gate_fail = w.gate_fail;
     o.min_wrap_dist = w.min_wrap; o.valid = 1; o.epoch = s.epoch;
     o.head = head; o.own_par = head & 1u;
@@ -1089,18 +1111,30 @@ BR_DEV bool br_predict_next_block(const BrStream& s, u32 b, const BrBlockIn& in,
 // cmd_blocks) and, at equal head parity, one bits_cur bitmap: each walk would read the other's fresh stored-bits as its own,
 // the commit would store their union, and the fixpoint could settle on bits no walk of the chunk produced (DESIGN.md
 // section 3).  So every chunk is walked at most once per launch, and a launch appends at most nblocks entries to ran_list.
-template <int G, bool M = false>
+//
+// The chunk records of the walk (br_walk_one) are kept in the warp's shared memory on the GPU: every lane writes the same
+// values, and a warp barrier lies between a record's last read and the next write over it.
+#define BR_WALK_WARPS 4   /* warps per block of k_walk */
+struct BrWalkRecs { BrBlockIn in, ni, used; BrBlockOut o; };
+template <int F, bool M = false>
 BR_DEV void br_walk_block(const BrStream& s, u32 b, bool to_block_end) {
   if (s.forced && !to_block_end && s.bin[b].blk == s.bin[s.counters[6]].blk) return;
-  BrBlockIn in = s.bin[b];
+#if BR_GPU
+  __shared__ BrWalkRecs recs[BR_WALK_WARPS];
+  BrWalkRecs& R = recs[threadIdx.x >> 5];
+#else
+  BrWalkRecs R;
+#endif
+  BrBlockIn& in = R.in;
+  BrBlockIn& ni = R.ni;
+  BrBlockOut& o = R.o;
+  in = s.bin[b];
   const u32 head = b;
   u32 sweep_p0 = 0xffffffffu;
   for (;;) {
-    BrBlockOut o;
-    br_walk_one<G, M>(s, b, in, o, head, sweep_p0);
+    br_walk_one<F, M>(s, b, in, o, head, sweep_p0, &R.used);
     if (br_lane() == 0) br_atomic_max((int*)s.counters + 16, (int)(b - head + 1));   // longest sweep of this launch (diagnostic)
     const u32 nb = b + 1;
-    BrBlockIn ni;
     if (in.last) {
       // block boundary: crossed by the sweeps of a sweep-mode launch, inside a group of sweep_blocks blocks
       const bool full_sweep = s.epoch > s.P.sweep_epoch + 9 && (s.epoch - 1 - s.P.sweep_epoch) % 3 == 0;   // (as br_chain_c decided it)
@@ -1147,6 +1181,8 @@ BR_DEV void br_walk_block(const BrStream& s, u32 b, bool to_block_end) {
 #endif
       br_syncwarp();
     }
+    br_syncwarp();
     in = ni; b = nb;
+    br_syncwarp();
   }
 }

@@ -217,14 +217,17 @@ static inline void br_bind_tables(BrStream& s, const u8* blob, const double* log
 #ifndef BR_WALK_G_SMALL
 #define BR_WALK_G_SMALL 1   /* rows fetched together for the 16/32-entry rings */
 #endif
-// Calls f(G, M) with the walker's template arguments for P as std::integral_constants: G the row grouping (0: the quick
-// search of qualities 2..4), M a batch of streams.
-template <int G, class F> static inline void br_walk_dispatch_m(const BrParams& P, F& f) {
-  if (P.multi) f(std::integral_constant<int, G>(), std::true_type());
-  else f(std::integral_constant<int, G>(), std::false_type());
+// Calls f(F, M) with the walker's template arguments for P as std::integral_constants: F the walker form (br_walk_form:
+// the row grouping, 0 for the quick search of qualities 2..4, and the ring size where it is fixed), M a batch of streams.
+// Quality 5 (16-entry ring) gets a form with the ring fixed; qualities 6..9 read it from P.  (A fixed 32-entry form for
+// quality 6 compiled with less spilling but walked 100 MB of text 5 % slower on an H100, DESIGN.md section 5.)
+template <int F, class Fn> static inline void br_walk_dispatch_m(const BrParams& P, Fn& f) {
+  if (P.multi) f(std::integral_constant<int, F>(), std::true_type());
+  else f(std::integral_constant<int, F>(), std::false_type());
 }
-template <class F> static inline void br_walk_dispatch(const BrParams& P, F&& f) {
+template <class Fn> static inline void br_walk_dispatch(const BrParams& P, Fn&& f) {
   if (P.quick) br_walk_dispatch_m<0>(P, f);
   else if (P.block_bits >= 6) br_walk_dispatch_m<BR_WALK_G_DEEP>(P, f);
+  else if (P.block_bits == 4) br_walk_dispatch_m<br_walk_form(BR_WALK_G_SMALL, 4)>(P, f);
   else br_walk_dispatch_m<BR_WALK_G_SMALL>(P, f);
 }

@@ -9,17 +9,16 @@
 // Its result, as many words: len, distance, score, delta, dl, dm, gate_checks, gate_fail, the own bit and the searched bit
 // the search set at cur, saw[0..3] (qualities 2..4; the slots a search does not read keep what the caller put there), 0, 0.
 // own: the walker's own bitmap (positions >= p0); the snapshot is s.bits_latest with its S-ordered copy s.storedS / s.prefS.
-// G == 0: the quick search of qualities 2..4.  Nothing is written to own or to the searched bitmap: a search's own writes
+// F: the walker form (br_walk_form), as br_walk_dispatch picks it; F == 0: the quick search of qualities 2..4.  Nothing is written to own or to the searched bitmap: a search's own writes
 // stay in the walker's gathered word, which is where the result reads them.
 #define BR_PROBE_WORDS 16
-template <int G>
+template <int F>
 BR_DEV void br_probe_search(const BrStream& s, u32* own, const u32* pr, u32* res) {
   const BrParams& P = s.P;
   BrWalk w;
   w.s = &s; w.d = s.data; w.p0 = pr[1]; w.base = pr[2]; w.pend = pr[3];
   w.own = own;
-  w.dict_l = ((u64)pr[13] << 32) | pr[12];
-  w.dict_m = ((u64)pr[15] << 32) | pr[14];
+  w.dict0 = pr + 12;
   w.dl = w.dm = w.gate_checks = w.gate_fail = 0;
   w.min_wrap = 0xffffffffu;
   w.fence_due = false;
@@ -32,8 +31,8 @@ BR_DEV void br_probe_search(const BrStream& s, u32* own, const u32* pr, u32* res
   for (int i = 0; i < 4; ++i) w.dc[i] = (int)pr[6 + i];
   const u32 cur = pr[0];
   BrSR sr; sr.len = pr[10]; sr.delta = 0; sr.distance = 0; sr.score = pr[11];
-  if constexpr (G == 0) br_find_quick(w, cur, w.pend - cur, pr[4], pr[5], sr);
-  else br_find_longest_match<G>(w, cur, w.pend - cur, pr[4], pr[5], sr, BrLook{cur + 1, cur + 2, 1});   // (with a lookahead, which must not change the result)
+  if constexpr (F == 0) br_find_quick(w, cur, w.pend - cur, pr[4], pr[5], sr);
+  else br_find_longest_match<F>(w, cur, w.pend - cur, pr[4], pr[5], sr, BrLook{cur + 1, cur + 2, 1});   // (with a lookahead, which must not change the result)
   if (br_lane() == 0) {
     const bool here = w.acc_wi == (cur >> 5);
     res[0] = sr.len; res[1] = sr.distance; res[2] = sr.score; res[3] = (u32)sr.delta;

@@ -64,6 +64,12 @@ struct BrParams {
 #define BR_CHUNK_BITS 11
 #define BR_CHUNK_BITS_SMALL 9
 #define BR_SMALL_STREAM (1u << 20)
+// The walker's compile-time form F (br_lz77.h, br_walk_dispatch): the row grouping G in the low byte (0: the quick search
+// of qualities 2..4) and above it the bucket ring's size as block_bits where it is fixed at compile time (0: P.block_bits,
+// read at run time).  A fixed ring lets quality 5 get a walker that holds only its own search paths.
+constexpr int br_walk_form(int G, int ring_bits) { return G | ring_bits << 8; }
+#define BR_FORM_G(F) ((F) & 0xff)
+#define BR_FORM_RB(F) ((F) >> 8)
 struct BrBlockIn {
   u32 pos, end;          // nominal slice [pos, end) of the input
   u32 blk_start, blk_end;  // the reference input block (one EncodeData call) that contains it
