@@ -73,3 +73,27 @@ BR_DEV void br_assemble_scan(const BrStream& s, const u64* out_off, u32* out, Br
   u64 total = (bit + 7) >> 3;
   res[0] = (u32)total; res[1] = (u32)(total >> 32); res[2] = fallbacks; res[3] = ncut;
 }
+// The copy of a descriptor goes word by word, in any order: br_copy_words words, word i by br_copy_word.  Bits: 32 from
+// outbits put at dst_bit + 32 i.  Raw bytes (byte aligned): the input bytes that fall into the i-th destination word.
+BR_DEV u32 br_copy_words(const BrCopyDesc& d) {
+  if (d.kind == 0) return (d.nbits + 31) / 32;
+  const u64 dst_byte = d.dst_bit >> 3;
+  return (u32)(((dst_byte + d.nbits - 1) >> 2) - (dst_byte >> 2) + 1);
+}
+BR_DEV void br_copy_word(const BrCopyDesc& d, u32 i, const u32* outbits, const u8* data, u32* out) {
+  if (d.kind == 0) {
+    u32 nb = (i + 1) * 32 <= d.nbits ? 32 : d.nbits - i * 32;
+    u32 v = outbits[d.src_off + i];
+    if (nb < 32) v &= (1u << nb) - 1;
+    u64 db = d.dst_bit + (u64)i * 32;
+    br_put_bits_at(out + (db >> 5), (u32)(db & 31), nb, v);
+  } else {
+    u64 dst_byte = d.dst_bit >> 3, first_word = dst_byte >> 2, wbyte = (first_word + i) << 2;
+    u32 v = 0;
+    for (u32 b = 0; b < 4; ++b) {
+      u64 ob = wbyte + b;
+      if (ob >= dst_byte && ob < dst_byte + d.nbits) v |= (u32)data[d.src_off + (ob - dst_byte)] << (8 * b);
+    }
+    if (v) br_atomic_or(out + first_word + i, v);
+  }
+}

@@ -1,11 +1,14 @@
 // br_kernels.cu -- CUDA kernels (sm_90a) and the per-stream pipeline that drives them.
 //
-// Stage map (reference function -> kernel):
-//   hash keys / bucket rings (hash_longest_match64_inc.h Store*)  -> br_build_index: k_radix_*, k_rank_compose, k_seg
-//   CreateBackwardReferences + FindLongestMatch                   -> k_walk      (one warp per input block)
-//   EncodeData glue (encode.c:985)                                -> k_chain     (one warp per stream)
-//   BrotliBuildMetaBlockGreedy + BrotliStoreMetaBlock             -> k_encode_mb (one warp per metablock)
-//   metablock concatenation / uncompressed fallback               -> k_assemble_scan, k_assemble_copy
+// Stages of job_compress: host functions that queue kernels on the job's stream and return false on a CUDA error (the
+// index and snapshot stages take any stream; the test hooks below call them too).
+//   stage_setup     arena, uploads, chunk table (k_build_chunks)
+//   stage_index     bucket rings (hash_longest_match64_inc.h Store*): br_build_index, k_slot_pred, k_tags
+//   stage_snapshot  the stored bits in S order and their prefix counts (k_build_storedS)
+//   stage_fixpoint  EncodeData glue (encode.c:985) k_chain_*, and CreateBackwardReferences / FindLongestMatch: k_walk
+//                   launches (a warp per scheduled chunk; k_cover, k_commit, k_verify, k_snapshot_update) to the fixpoint
+//   stage_entropy   BrotliBuildMetaBlockGreedy + BrotliStoreMetaBlock: k_compact, E0..E7 (br_entropy2.h)
+//   stage_assemble  metablock concatenation and the late uncompressed fallback: k_assemble_scan, k_assemble_copy
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -174,15 +177,10 @@ static void radix_pass(Keys keys, const u32* vals, u32 n, u32* hist, u32* scan_t
   scan_exclusive(hist, 256 * ntiles, scan_tmp, st);
   k_radix_scatter<SHIFT, HAS_VALS, KT><<<ntiles, RADIX_THREADS, smem, st>>>(keys, vals, n, hist, ntiles, out_keys, out_vals, rk);
 }
-// chunk table of one input block (what br_build_blocks would fill on the host): one CTA per block
+// chunk table of one input block (br_params.h br_chunk_in): one CTA per block
 __global__ void k_build_chunks(const BrBlk* __restrict__ blk, BrBlockIn* __restrict__ bin, u32 ch) {
   const BrBlk B = blk[blockIdx.x];
-  for (u32 c = threadIdx.x; c < B.nchunks; c += blockDim.x) {
-    BrBlockIn k; memset(&k, 0, sizeof(k));
-    k.pos = B.start + c * ch; k.end = k.pos + ch < B.end ? k.pos + ch : B.end; k.blk_start = B.start; k.blk_end = B.end;
-    k.first = c == 0; k.last = k.end == B.end; k.is_last = B.is_last; k.force_flush = B.force_flush; k.blk = blockIdx.x; k.base = B.base;
-    bin[B.first_chunk + c] = k;
-  }
+  for (u32 c = threadIdx.x; c < B.nchunks; c += blockDim.x) bin[B.first_chunk + c] = br_chunk_in(B, blockIdx.x, c, ch);
 }
 // tagS[j] = tag of the position S[j] (br_lz77.h br_tag4)
 __global__ void k_tags(const u8* __restrict__ data, const u32* __restrict__ S, u32 n, u16* __restrict__ tagS) {
@@ -465,37 +463,13 @@ __global__ void k_assemble_scan(BrStream s, const u64* __restrict__ out_off, u32
                                 int with_header, const u32* __restrict__ cut_kind, u64* cut_end_bit, u64* stream_end) {
   if (threadIdx.x == 0) br_assemble_scan(s, out_off, out, desc, res, with_header, cut_kind, cut_end_bit, stream_end);
 }
-// grid.y = metablock, grid.x strides over its words / bytes
+// grid.y = metablock, grid.x strides over its words (br_assemble.h br_copy_word)
 __global__ void k_assemble_copy(BrStream s, const BrCopyDesc* __restrict__ desc, const u32* __restrict__ outbits, u32* out, u32 n_mbs) {
   for (u32 m = blockIdx.y; m < n_mbs; m += gridDim.y) {   // (grid.y is capped at 65535, see k_cmd_mb)
-  const BrCopyDesc d = desc[m];
-  if (d.kind == 0) {
-    u32 nwords = (d.nbits + 31) / 32;
-    const u32* src = outbits + d.src_off;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < nwords; i += gridDim.x * blockDim.x) {
-      u32 nb = (i + 1) * 32 <= d.nbits ? 32 : d.nbits - i * 32;
-      u32 v = src[i];
-      if (nb < 32) v &= (1u << nb) - 1;
-      u64 db = d.dst_bit + (u64)i * 32;
-      br_put_bits_at(out + (db >> 5), (u32)(db & 31), nb, v);
-    }
-  } else {
-    // raw bytes: destination is byte aligned; go through 32-bit words of the destination
-    u64 dst_byte = d.dst_bit >> 3;
-    u32 nbytes = d.nbits;
-    u64 first_word = dst_byte >> 2, last_word = (dst_byte + nbytes - 1) >> 2;
-    u32 nw = (u32)(last_word - first_word + 1);
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < nw; i += gridDim.x * blockDim.x) {
-      u64 wbyte = (first_word + i) << 2;
-      u32 v = 0;
-      for (u32 b = 0; b < 4; ++b) {
-        u64 ob = wbyte + b;
-        if (ob >= dst_byte && ob < dst_byte + nbytes) v |= (u32)s.data[d.src_off + (ob - dst_byte)] << (8 * b);
-      }
-      if (v) atomicOr(out + first_word + i, v);
-    }
+    const BrCopyDesc d = desc[m];
+    const u32 nw = br_copy_words(d);
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < nw; i += gridDim.x * blockDim.x) br_copy_word(d, i, outbits, s.data, out);
   }
-}
 }
 
 // ============================================================================ host pipeline
@@ -634,6 +608,254 @@ static void carve_index_quick(BrCarve& A, const BrParams& P, BrIndexBufs& b) {
   b.qk_keys = A.take<u32>(n + 4); b.qk_K1 = A.take<u32>(n + 4); b.qk_V1 = A.take<u32>(n + 4); b.qk_V2 = A.take<u32>(n + 4);
 }
 
+// The job's device arrays that BrStream does not hold.  Main arena (stage_setup): the index's sort buffers, the stored
+// bits of every 1024 positions of S (cntS, scanned into prefS with scan_tmp2) and the cut and stream-end records.
+// arena2 (carve_entropy): the entropy stage's arrays and the assembled output.
+struct BrJobBufs {
+  BrIndexBufs ix; u32 *cntS, *scan_tmp2, *cut_kind; u64 *cut_end, *stream_end;
+  BrEnt e; u32 *out, *res, *code_base, *stmp; BrCopyDesc* desc; BrHTree* tree_pool;
+};
+// arena2 in arena order: the metablocks' scratch and bit buffers (L), the output, and the entropy stage's arrays for C
+// commands over n input bytes.  e gets every array and zero totals.  pool_workers: the E4 thread workers that the tree
+// pool holds a tree area for.
+static void carve_entropy(BrCarve& B, const BrMbLayout& L, size_t n, size_t C, size_t pool_workers, BrJobBufs& b) {
+  const size_t n_mbs = L.scratch_off.size();
+  BrEnt& e = b.e;
+  memset(&e, 0, sizeof(e));
+  e.scratch = B.take<u8>(L.scratch_bytes + 256); e.outbits = B.take<u32>(L.out_words + 64);
+  b.out = B.take<u32>(L.out_cap / 4 + 16); e.cmds = B.take<BrCmd>(C + 1);
+  e.scratch_off = B.take<u64>(n_mbs); e.out_off = B.take<u64>(n_mbs);
+  b.desc = B.take<BrCopyDesc>(n_mbs); b.res = B.take<u32>(16);
+  e.lit_ord = B.take<u32>(C + 2); e.cmd_pos = B.take<u32>(C + 2); e.dist_ord = B.take<u32>(C + 2);
+  e.cmd_len = B.take<u32>(C + 2); e.lit_bit_base = B.take<u32>(C + 2); e.cmd_mb = B.take<u32>(C + 2);
+  e.dist_sym = B.take<u16>(C + 2);
+  e.lit_pos = B.take<u32>(n + 2); e.lit_cmd = B.take<u32>(n + 2); e.lit_len = B.take<u32>(n + 2);
+  e.aux = B.take<BrMbAux>(n_mbs);
+  b.code_base = B.take<u32>(n_mbs + 1);
+  b.tree_pool = B.take<BrHTree>(pool_workers * BR_CODE_TREE_NODES);
+  b.stmp = B.take<u32>(scan_tmp_words(n + C + 8) * 2);
+}
+// E0 and E1 (br_entropy2.h) over the C commands of e: their ordinals with the totals read back into e (through `totals`,
+// two host words), each command's metablock, each literal's position and command.  False on a CUDA error or on more
+// literals than input bytes.
+static bool launch_e01(const BrStream& s, BrEnt& e, u32 C, u32 n_mbs, u32* stmp, u32* totals, cudaStream_t st) {
+  e.total_cmds = C;
+  u32 *lit_ord = (u32*)e.lit_ord, *cmd_pos = (u32*)e.cmd_pos, *dist_ord = (u32*)e.dist_ord;
+  k_cmd_scan_inputs<<<(C + 1 + 255) / 256, 256, 0, st>>>(e.cmds, C, lit_ord, cmd_pos, dist_ord);
+  scan_exclusive(lit_ord, C + 1, stmp, st);
+  scan_exclusive(cmd_pos, C + 1, stmp, st);
+  scan_exclusive(dist_ord, C + 1, stmp, st);
+  CK(cudaMemcpyAsync(totals, lit_ord + C, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(totals + 1, dist_ord + C, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  e.total_lits = totals[0]; e.total_dist = totals[1];
+  if (e.total_lits > s.P.n) return false;
+  k_cmd_mb<<<dim3(64, n_mbs < 65535u ? n_mbs : 65535u), 256, 0, st>>>(s, e.cmd_mb, n_mbs);
+  k_expand<<<(C + 127) / 128 + 1, 128, 0, st>>>(e);
+  return true;
+}
+
+// Setup: the main arena carved (s's arrays, b's), the input and the plan's tables uploaded, the chunk table built and the
+// fixpoint's state cleared.  s.P: the plan's parameters.
+static bool stage_setup(BrJob* job, BrStream& s, const BrDeviceTables* T, const BrStreamPlan& plan, const BrCuts* cuts,
+                        const u8* d_in, BrJobBufs& b) {
+  const BrParams& P = s.P;
+  const u32 n = P.n, nb = P.nblocks, nblk = (u32)plan.blk.size(), ncuts = cuts ? cuts->n : 0, nstreams = plan.nstreams;
+  const size_t nwords = (size_t)(n + 31) / 32 + 2;
+  cudaStream_t st = job->st;
+  s.bits_words = (u32)nwords; s.cmd_stride = plan.cmd_stride; s.nblk = nblk;
+  auto carve = [&](BrCarve& A) {
+    s.data = A.take<u8>((size_t)n + 64);
+    carve_index(A, P, b.ix);
+    s.bits_latest = A.take<u32>(nwords); s.bits_cur = A.take<u32>(2 * nwords);
+    s.srch_latest = A.take<u32>(nwords); s.srch_cur = A.take<u32>(nwords); s.bits_prev = A.take<u32>(nwords);
+    s.cover_cur = A.take<u32>(nwords);
+    s.storedS = A.take<u32>(nwords + 64); s.prefS = A.take<u32>((size_t)n / 1024 + 8); b.cntS = A.take<u32>((size_t)n / 1024 + 8);
+    b.scan_tmp2 = A.take<u32>(scan_tmp_words((size_t)n / 1024 + 8));
+    s.bin = A.take<BrBlockIn>(nb); s.bin_used = A.take<BrBlockIn>(nb);
+    s.bout = A.take<BrBlockOut>(nb);
+    s.cmd_blocks = A.take<BrCmd>((size_t)nb * plan.cmd_stride);
+    s.dirty = A.take<u32>(nb + 16); s.changed_bits = A.take<u32>(nb + 16);
+    s.changed_epoch = A.take<int>(nb + 16); s.ext_total = A.take<u32>(nb + 16);
+    s.cmd_off = A.take<u32>(nb + 16); s.force_unc = A.take<u32>(nb + 16);
+    s.dirty_list = A.take<u32>(nb + 16); s.block_mb = A.take<u32>(nb + 16);
+    s.ran_list = A.take<u32>(plan.ran_cap); s.lil_in = A.take<u32>(nb + 16);
+    s.bitdep_epoch = A.take<int>(nb + 16);
+    s.blk = A.take<BrBlk>(nblk); s.blkin = A.take<BrBlkIn>(nblk);
+    s.key_flips = A.take<u32>(P.nbuckets + 8);
+    s.slot_blk = A.take<u32>(plan.slot_blk.size()); b.cut_kind = A.take<u32>(ncuts + 2); b.cut_end = A.take<u64>(ncuts + 2);
+    b.stream_end = A.take<u64>(nstreams + 2);
+    s.epoch_cum = A.take<u32>((size_t)P.max_epochs + 2);
+    s.mbs = A.take<BrMetaBlock>(nb + 1);
+    s.stream_blk = A.take<u32>(nstreams + 2); s.stream_nmb = A.take<u32>(nstreams + 2); s.stream_ncmd = A.take<u32>(nstreams + 2);
+    s.mbs_stage = A.take<BrMetaBlock>(nblk);
+    s.counters = A.take<u32>(64); s.hist_scratch = A.take<u32>(256ull * nstreams);
+    if (P.quick) {   // 32-bit sort keys, slot reads, slot entry points
+      carve_index_quick(A, P, b.ix);
+      s.saw = A.take<u32>(((size_t)n << P.qk_sweep_bits) + 16);
+      s.qpred = A.take<u32>(((size_t)n << P.qk_sweep_bits) + 16);
+    }
+  };
+  if (!br_carve(job->arena, carve)) return false;
+  s.S = b.ix.S; s.rank = b.ix.rank; s.seg = b.ix.seg; s.skeys = b.ix.K2; s.tagS = b.ix.tagS;
+  br_bind_tables(s, T->blob, T->log2tab, T->log2tab_n);
+
+  CK(cudaMemcpyAsync((u8*)s.data, d_in, n, cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemsetAsync((u8*)s.data + n, 0, 64, st));
+  CK(cudaMemcpyAsync(s.blk, plan.blk.data(), nblk * sizeof(BrBlk), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync((u32*)s.slot_blk, plan.slot_blk.data(), plan.slot_blk.size() * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync((u32*)s.stream_blk, plan.stream_blk.data(), (nstreams + 1) * 4ull, cudaMemcpyHostToDevice, st));
+  if (ncuts) CK(cudaMemcpyAsync(b.cut_kind, cuts->kind, ncuts * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(s.bin, 0, nb * sizeof(BrBlockIn), st));
+  k_build_chunks<<<nblk, 64, 0, st>>>(s.blk, s.bin, 1u << P.chunk_bits);
+  CK(cudaStreamSynchronize(st));   // (the copies from the plan's host tables must be done before the arrays below are reused)
+  CK(cudaMemsetAsync(s.bout, 0, nb * sizeof(BrBlockOut), st));
+  CK(cudaMemsetAsync(s.bin_used, 0, nb * sizeof(BrBlockIn), st));
+  CK(cudaMemsetAsync(s.changed_bits, 0, (nb + 16) * 4, st));
+  CK(cudaMemsetAsync(s.changed_epoch, 0xFF, (nb + 16) * 4, st));
+  CK(cudaMemsetAsync(s.bitdep_epoch, 0xFF, (nb + 16) * 4, st));
+  CK(cudaMemsetAsync(s.srch_latest, 0, nwords * 4, st));
+  CK(cudaMemsetAsync(s.key_flips, 0, (P.nbuckets + 8) * 4, st));
+  CK(cudaMemsetAsync(s.force_unc, 0, (nb + 16) * 4, st));
+  CK(cudaMemsetAsync(s.epoch_cum, 0, 64, st));
+  CK(cudaMemsetAsync(s.counters, 0, 256, st));
+  CK(cudaMemsetAsync(s.bits_cur, 0, 2 * (size_t)nwords * 4, st));
+  return true;
+}
+// Index: S, rank and seg (br_build_index), at qualities 2..4 the slot entry points, and tagS when `tags`.
+static void stage_index(const BrStream& s, const BrIndexBufs& ix, bool tags, cudaStream_t st) {
+  br_build_index(s.P, s.data, s.blk, s.nblk, ix, st);
+  if (s.P.quick) k_slot_pred<<<s.nblk, 256, 0, st>>>(s, (u32*)s.qpred);   // (the kernel reads s.S / s.rank / s.seg / s.blk / s.data only)
+  if (tags) k_tags<<<(s.P.n + 255) / 256, 256, 0, st>>>(s.data, ix.S, s.P.n, ix.tagS);
+}
+// prefS = the exclusive scan of cntS, the stored bits of every 1024 positions of S
+static void refresh_prefS(const BrStream& s, const u32* cntS, u32* scan_tmp2, cudaStream_t st) {
+  const u32 nsnap = (s.P.n + 1023) / 1024;
+  cudaMemcpyAsync((u32*)s.prefS, cntS, nsnap * 4ull, cudaMemcpyDeviceToDevice, st);
+  scan_exclusive((u32*)s.prefS, nsnap, scan_tmp2, st);
+}
+// Snapshot: bits_latest in S order (storedS) and its prefix counts (prefS), for the bucket rings of qualities 5..9.  Built
+// once; the fixpoint carries it along after every launch's commits (k_snapshot_update).
+static void stage_snapshot(const BrStream& s, u32* cntS, u32* scan_tmp2, cudaStream_t st) {
+  k_build_storedS<<<(s.P.n + 1023) / 1024, 1024, 0, st>>>(s, (u32*)s.storedS, cntS);
+  refresh_prefS(s, cntS, scan_tmp2, st);
+}
+// Fixpoint: the chain, then walk launches until no chunk is dirty.  *n_mbs, *total_cmds: the metablocks and commands of
+// the parse it settles on.  trace (BR_DEBUG_KNOBS builds): every launch, then the slowest chunk walks, on stderr.
+static bool stage_fixpoint(BrJob* job, BrStream& s, const BrJobBufs& b, bool trace, u32* n_mbs, u32* total_cmds) {
+  const BrParams& P = s.P;
+  const u32 nb = P.nblocks, nblk = s.nblk, ch = 1u << P.chunk_bits, nwords = s.bits_words;
+  cudaStream_t st = job->st; cudaEvent_t* ev = job->ev; u32* hp = job->h_pinned;
+  const u32 round_epoch0 = s.epoch;
+  bool walk_pending = false;
+  for (;;) {
+    k_chain_a<<<(nblk + 31) / 32, 32, 0, st>>>(s);
+    if (P.multi) {
+      k_chain_b1<<<(P.multi + 3) / 4, 128, 0, st>>>(s);
+      k_chain_b2<<<1, 32, 0, st>>>(s);
+      k_chain_b3<<<(nblk + 255) / 256, 256, 0, st>>>(s);
+    } else k_chain_b<<<1, 32, 0, st>>>(s);
+    k_chain_c<<<(nblk + 31) / 32, 32, 0, st>>>(s);
+    k_chain_d<<<(nb + 255) / 256, 256, 0, st>>>(s);
+    CK(cudaMemcpyAsync(hp, s.counters, 128, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    u32 n_dirty = hp[0], n_sched = hp[5]; *n_mbs = hp[1]; *total_cmds = hp[2];
+    job->stats.block_runs += hp[4];
+    if (hp[4] > job->stats.max_walks) job->stats.max_walks = hp[4];
+    if (trace) fprintf(stderr, "epoch %u: dirty %u sched %u ran %u longest sweep %u | never %u state %u dict %u bits %u wrap %u\n", s.epoch, hp[0], hp[5], hp[4], hp[16], hp[9], hp[10], hp[11], hp[12], hp[13]);
+    if (walk_pending) {
+      float wms; cudaEventElapsedTime(&wms, ev[6], ev[7]); job->stats.ms_walk += wms; walk_pending = false;
+      if (trace) fprintf(stderr, "   walk launch %u: %.2f ms\n", s.epoch, wms);
+    }
+    if (n_dirty == 0) break;
+    if (s.epoch + 2 >= P.max_epochs) { fprintf(stderr, "brotli_b200: internal error: launch bound exceeded\n"); return false; }
+    ++s.epoch; ++job->stats.lz77_iterations;
+    s.forced = s.epoch - round_epoch0 >= P.force_epoch ? 1u : 0u;
+    job->stats.forced_launches += s.forced;
+    CK(cudaMemsetAsync(s.bits_cur, 0, 2 * (size_t)nwords * 4, st));
+    CK(cudaMemsetAsync(s.srch_cur, 0, nwords * 4, st));
+    CK(cudaMemsetAsync(s.counters + 4, 0, 4, st));
+    CK(cudaMemsetAsync(s.counters + 16, 0, 4, st));
+    cudaEventRecord(ev[6], st);
+    const u32 wg = (n_sched + BR_WALK_WARPS - 1) / BR_WALK_WARPS;
+    br_walk_dispatch(P, [&](auto g, auto m) { k_walk<decltype(g)::value, decltype(m)::value><<<wg, 32 * BR_WALK_WARPS, 0, st>>>(s); });
+    cudaEventRecord(ev[7], st);
+    walk_pending = true; ++job->stats.walk_launches; job->stats.launches += 6;
+    job->stats.walk_bytes += (u64)n_sched * ch;
+    CK(cudaMemcpyAsync((u32*)s.bits_prev, s.bits_latest, nwords * 4, cudaMemcpyDeviceToDevice, st));
+    if (!P.quick) {   // (quality 2..4 check every run instead of marking: br_verify_run)
+      CK(cudaMemsetAsync(s.cover_cur, 0, nwords * 4, st));
+      k_cover<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s);
+    }
+    k_commit<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s);
+    if (P.quick) k_verify<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s);
+    else {
+      k_snapshot_update<<<(u32)((nwords + 255) / 256), 256, 0, st>>>(s, (u32*)s.storedS, b.cntS);
+      refresh_prefS(s, b.cntS, b.scan_tmp2, st);
+    }
+  }
+  cudaEventRecord(ev[2], st);
+#ifdef BR_DEBUG_KNOBS
+  if (trace) {   // the slowest chunk walks of the final state, and a per-megabyte profile
+    std::vector<BrBlockOut> hb2(nb);
+    cudaMemcpyAsync(hb2.data(), s.bout, nb * sizeof(BrBlockOut), cudaMemcpyDeviceToHost, st); cudaStreamSynchronize(st);
+    const u32 per = (1u << 20) >> P.chunk_bits;
+    for (u32 a = 0; a < nb; a += per) {
+      unsigned long long cyc = 0, se = 0, ro = 0; u32 mx = 0;
+      for (u32 k = a; k < a + per && k < nb; ++k) { cyc += hb2[k].dbg_kcycles; se += hb2[k].dbg_searches; ro += hb2[k].dbg_rows; if (hb2[k].dbg_kcycles > mx) mx = hb2[k].dbg_kcycles; }
+      fprintf(stderr, "MiB %4u: %7.2f Mcycles per chunk (max %7.2f)  searches/chunk %5llu rows/search %5.1f\n", a / per, cyc / 1024.0 / per, mx / 1024.0, se / per, se ? (double)ro / se : 0.0);
+    }
+  }
+#endif
+  return true;
+}
+// Entropy: the metablocks' layout, arena2 (carve_entropy), the compacted commands and E0..E7 (br_entropy2.h): every
+// compressed metablock's bits in its buffer.
+static bool stage_entropy(BrJob* job, const BrStream& s, BrJobBufs& b, u32 n_mbs, u32 C) {
+  const BrParams& P = s.P;
+  cudaStream_t st = job->st;
+  std::vector<BrMetaBlock> hm(n_mbs);
+  CK(cudaMemcpyAsync(hm.data(), s.mbs, n_mbs * sizeof(BrMetaBlock), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  BrMbLayout L;
+  br_mb_layout(P, hm.data(), n_mbs, L);
+  if (!br_carve(job->arena2, [&](BrCarve& B) { carve_entropy(B, L, P.n, C, (L.code_workers + 63) & ~63u, b); })) return false;
+  BrEnt& e = b.e;
+  CK(cudaMemcpyAsync((u64*)e.scratch_off, L.scratch_off.data(), n_mbs * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync((u64*)e.out_off, L.out_off.data(), n_mbs * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(e.outbits, 0, (L.out_words + 64) * 4, st));
+  CK(cudaMemsetAsync(b.out, 0, L.out_cap + 64, st));
+  k_compact<<<(P.nblocks * 32 + 127) / 128, 128, 0, st>>>(s, (BrCmd*)e.cmds, s.block_mb);
+  cudaEventRecord(job->ev[8], st);
+  if (!launch_e01(s, e, C, n_mbs, b.stmp, job->h_pinned + 24, st) || !launch_split(s, e, n_mbs, st)) return false;
+  if (P.mb_kind) k_prep_flat<<<n_mbs, 64, 0, st>>>(s, e);   // qualities 2, 3: no block split, one code per category
+  else launch_codes(s, e, L, n_mbs, b.code_base, b.stmp, b.tree_pool, 0, st);
+  k_lit_bits<<<(e.total_lits + 1 + 255) / 256, 256, 0, st>>>(s, e);
+  k_cmd_bits<<<(C + 1 + 255) / 256, 256, 0, st>>>(s, e);
+  scan_exclusive(e.lit_len, e.total_lits + 1, b.stmp, st);
+  scan_exclusive(e.cmd_len, C + 1, b.stmp, st);
+  k_emit_cmd<<<(C + 255) / 256, 256, 0, st>>>(s, e);
+  if (e.total_lits) k_emit_lit<<<(e.total_lits + 255) / 256, 256, 0, st>>>(s, e);
+  cudaEventRecord(job->ev[9], st);
+  return true;
+}
+
+// Assembly: where every metablock's bits go (k_assemble_scan).  *redo: a coded metablock is larger than its input, so
+// it is stored raw (encode.c:604; br_assemble_scan marked it in force_unc) and the parse behind it must be redone with
+// the restored distance cache; nothing is copied then.  Otherwise the copies, and *out / *size: the stream.
+static bool stage_assemble(BrJob* job, const BrStream& s, const BrJobBufs& b, int with_header, u32 n_mbs, bool* redo,
+                           const u8** out, size_t* size) {
+  cudaStream_t st = job->st; u32* hp = job->h_pinned;
+  k_assemble_scan<<<1, 32, 0, st>>>(s, b.e.out_off, b.out, b.desc, b.res, with_header, b.cut_kind, b.cut_end, b.stream_end);
+  CK(cudaMemcpyAsync(hp + 16, b.res, 16, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  *redo = hp[18] != 0;
+  if (*redo) return true;
+  k_assemble_copy<<<dim3(64, n_mbs < 65535u ? n_mbs : 65535u), 256, 0, st>>>(s, b.desc, b.e.outbits, b.out, n_mbs);
+  *out = (const u8*)b.out; *size = ((u64)hp[17] << 32) | hp[16];
+  return true;
+}
+
 // Compress one stream whose input already sits in device memory (d_in, n bytes).  The
 // compressed bytes are left in device memory (*d_out, *out_size; valid until the next call on
 // this job).  Returns 1 on success, 0 on failure (unsupported parameters, CUDA error).
@@ -657,234 +879,34 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
 #else
   const bool trace = false;
 #endif
-  const u32 nb = P.nblocks, nblk = (u32)plan.blk.size(), ncuts = cuts ? cuts->n : 0, nstreams = plan.nstreams;
-  const u32 ch = 1u << P.chunk_bits;
+  const u32 ncuts = cuts ? cuts->n : 0, nstreams = plan.nstreams;
   cudaStream_t st = job->st;
   memset(&job->stats, 0, sizeof(job->stats));
   job->stats.ran_cap = plan.ran_cap;
   cudaEvent_t* ev = job->ev;
   cudaEventRecord(ev[0], st);
-
-  const size_t nwords = (size_t)(n + 31) / 32 + 2;
-  s.bits_words = (u32)nwords; s.cmd_stride = plan.cmd_stride; s.nblk = nblk;
-  BrIndexBufs ix;
-  u32 *cntS, *scan_tmp2, *cut_kind;
-  u64 *cut_end, *stream_end;
-  auto carve = [&](BrCarve& A) {
-    s.data = A.take<u8>((size_t)n + 64);
-    carve_index(A, P, ix);
-    s.bits_latest = A.take<u32>(nwords); s.bits_cur = A.take<u32>(2 * nwords);
-    s.srch_latest = A.take<u32>(nwords); s.srch_cur = A.take<u32>(nwords); s.bits_prev = A.take<u32>(nwords);
-    s.cover_cur = A.take<u32>(nwords);
-    s.storedS = A.take<u32>(nwords + 64); s.prefS = A.take<u32>((size_t)n / 1024 + 8); cntS = A.take<u32>((size_t)n / 1024 + 8);
-    scan_tmp2 = A.take<u32>(scan_tmp_words((size_t)n / 1024 + 8));
-    s.bin = A.take<BrBlockIn>(nb); s.bin_used = A.take<BrBlockIn>(nb);
-    s.bout = A.take<BrBlockOut>(nb);
-    s.cmd_blocks = A.take<BrCmd>((size_t)nb * plan.cmd_stride);
-    s.dirty = A.take<u32>(nb + 16); s.changed_bits = A.take<u32>(nb + 16);
-    s.changed_epoch = A.take<int>(nb + 16); s.ext_total = A.take<u32>(nb + 16);
-    s.cmd_off = A.take<u32>(nb + 16); s.force_unc = A.take<u32>(nb + 16);
-    s.dirty_list = A.take<u32>(nb + 16); s.block_mb = A.take<u32>(nb + 16);
-    s.ran_list = A.take<u32>(plan.ran_cap); s.lil_in = A.take<u32>(nb + 16);
-    s.bitdep_epoch = A.take<int>(nb + 16);
-    s.blk = A.take<BrBlk>(nblk); s.blkin = A.take<BrBlkIn>(nblk);
-    s.key_flips = A.take<u32>(P.nbuckets + 8);
-    s.slot_blk = A.take<u32>(plan.slot_blk.size()); cut_kind = A.take<u32>(ncuts + 2); cut_end = A.take<u64>(ncuts + 2);
-    stream_end = A.take<u64>(nstreams + 2);
-    s.epoch_cum = A.take<u32>((size_t)P.max_epochs + 2);
-    s.mbs = A.take<BrMetaBlock>(nb + 1);
-    s.stream_blk = A.take<u32>(nstreams + 2); s.stream_nmb = A.take<u32>(nstreams + 2); s.stream_ncmd = A.take<u32>(nstreams + 2);
-    s.mbs_stage = A.take<BrMetaBlock>(nblk);
-    s.counters = A.take<u32>(64); s.hist_scratch = A.take<u32>(256ull * nstreams);
-    if (P.quick) {   // 32-bit sort keys, slot reads, slot entry points
-      carve_index_quick(A, P, ix);
-      s.saw = A.take<u32>(((size_t)n << P.qk_sweep_bits) + 16);
-      s.qpred = A.take<u32>(((size_t)n << P.qk_sweep_bits) + 16);
-    }
-  };
-  if (!br_carve(job->arena, carve)) return 0;
-  s.S = ix.S; s.rank = ix.rank; s.seg = ix.seg; s.skeys = ix.K2; s.tagS = ix.tagS;
-  br_bind_tables(s, T->blob, T->log2tab, T->log2tab_n);
-
-  CK(cudaMemcpyAsync((u8*)s.data, d_in, n, cudaMemcpyDeviceToDevice, st));
-  CK(cudaMemsetAsync((u8*)s.data + n, 0, 64, st));
-  CK(cudaMemcpyAsync(s.blk, plan.blk.data(), nblk * sizeof(BrBlk), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync((u32*)s.slot_blk, plan.slot_blk.data(), plan.slot_blk.size() * 4, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync((u32*)s.stream_blk, plan.stream_blk.data(), (nstreams + 1) * 4ull, cudaMemcpyHostToDevice, st));
-  if (ncuts) CK(cudaMemcpyAsync(cut_kind, cuts->kind, ncuts * 4, cudaMemcpyHostToDevice, st));
-  CK(cudaMemsetAsync(s.bin, 0, nb * sizeof(BrBlockIn), st));
-  k_build_chunks<<<nblk, 64, 0, st>>>(s.blk, s.bin, ch);
-  CK(cudaStreamSynchronize(st));   // (the copies from the plan's host tables must be done before the arrays below are reused)
-  CK(cudaMemsetAsync(s.bout, 0, nb * sizeof(BrBlockOut), st));
-  CK(cudaMemsetAsync(s.bin_used, 0, nb * sizeof(BrBlockIn), st));
-  CK(cudaMemsetAsync(s.changed_bits, 0, (nb + 16) * 4, st));
-  CK(cudaMemsetAsync(s.changed_epoch, 0xFF, (nb + 16) * 4, st));
-  CK(cudaMemsetAsync(s.bitdep_epoch, 0xFF, (nb + 16) * 4, st));
-  CK(cudaMemsetAsync(s.srch_latest, 0, nwords * 4, st));
-  CK(cudaMemsetAsync(s.key_flips, 0, (P.nbuckets + 8) * 4, st));
-  CK(cudaMemsetAsync(s.force_unc, 0, (nb + 16) * 4, st));
-  CK(cudaMemsetAsync(s.epoch_cum, 0, 64, st));
-  CK(cudaMemsetAsync(s.counters, 0, 256, st));
-  CK(cudaMemsetAsync(s.bits_cur, 0, 2 * (size_t)nwords * 4, st));
-
-  // ---- position index: S, rank, seg
-  br_build_index(P, s.data, s.blk, nblk, ix, st);
-  if (P.quick) k_slot_pred<<<nblk, 256, 0, st>>>(s, (u32*)s.qpred);   // (the kernel reads s.S / s.rank / s.seg / s.blk / s.data only)
+  BrJobBufs b;
+  if (!stage_setup(job, s, T, plan, cuts, d_in, b)) return 0;
   // (the 16/32-entry rings of quality 5-6 gained nothing from tags when timed on C2, so only the deep rings of quality 7-9,
   // where most of the 256 ring entries are hash collisions whose bytes need not be fetched, use them)
-  if (P.block_bits >= 6) k_tags<<<(n + 255) / 256, 256, 0, st>>>(s.data, ix.S, n, ix.tagS);
-  CK(cudaMemsetAsync(s.bits_latest, 0, nwords * 4, st));
-  k_init_bits<<<nblk, 256, 0, st>>>(s);
+  stage_index(s, b.ix, P.block_bits >= 6, st);
+  CK(cudaMemsetAsync(s.bits_latest, 0, s.bits_words * 4ull, st));
+  k_init_bits<<<s.nblk, 256, 0, st>>>(s);
   cudaEventRecord(ev[1], st);
-  // the S-ordered snapshot of the stored bits, for the bucket rings of quality 5..9: built once here, then carried along by
-  // k_snapshot_update after every launch's commits
-  const u32 nsnap = (n + 1023) / 1024;
-  u32* const storedS = (u32*)s.storedS;
-  u32* const prefS = (u32*)s.prefS;
-  auto refresh_prefS = [&]() {
-    cudaMemcpyAsync(prefS, cntS, nsnap * 4ull, cudaMemcpyDeviceToDevice, st);
-    scan_exclusive(prefS, nsnap, scan_tmp2, st);
-  };
-  if (!P.quick) {
-    k_build_storedS<<<nsnap, 1024, 0, st>>>(s, storedS, cntS);
-    refresh_prefS();
-  }
+  if (!P.quick) stage_snapshot(s, b.cntS, b.scan_tmp2, st);
 
-  // ---- LZ77 fixpoint
-  u32* hp = job->h_pinned;
   u32 n_mbs = 0, total_cmds = 0;
   int rounds = 0;
-  bool walk_pending = false;
   const u8* final_out = nullptr; size_t final_size = 0;
   for (;;) {   // rounds: repeated only when a metablock needs the late uncompressed fallback
     ++rounds;
-    const u32 round_epoch0 = s.epoch;
-    for (;;) {
-      k_chain_a<<<(nblk + 31) / 32, 32, 0, st>>>(s);
-      if (P.multi) {
-        k_chain_b1<<<(P.multi + 3) / 4, 128, 0, st>>>(s);
-        k_chain_b2<<<1, 32, 0, st>>>(s);
-        k_chain_b3<<<(nblk + 255) / 256, 256, 0, st>>>(s);
-      } else k_chain_b<<<1, 32, 0, st>>>(s);
-      k_chain_c<<<(nblk + 31) / 32, 32, 0, st>>>(s);
-      k_chain_d<<<(nb + 255) / 256, 256, 0, st>>>(s);
-      CK(cudaMemcpyAsync(hp, s.counters, 128, cudaMemcpyDeviceToHost, st));
-      CK(cudaStreamSynchronize(st));
-      u32 n_dirty = hp[0], n_sched = hp[5]; n_mbs = hp[1]; total_cmds = hp[2];
-      job->stats.block_runs += hp[4];
-      if (hp[4] > job->stats.max_walks) job->stats.max_walks = hp[4];
-      if (trace) fprintf(stderr, "epoch %u: dirty %u sched %u ran %u longest sweep %u | never %u state %u dict %u bits %u wrap %u\n", s.epoch, hp[0], hp[5], hp[4], hp[16], hp[9], hp[10], hp[11], hp[12], hp[13]);
-      if (walk_pending) {
-        float wms; cudaEventElapsedTime(&wms, ev[6], ev[7]); job->stats.ms_walk += wms; walk_pending = false;
-        if (trace) fprintf(stderr, "   walk launch %u: %.2f ms\n", s.epoch, wms);
-      }
-      if (n_dirty == 0) break;
-      if (s.epoch + 2 >= P.max_epochs) { fprintf(stderr, "brotli_b200: internal error: launch bound exceeded\n"); return 0; }
-      ++s.epoch; ++job->stats.lz77_iterations;
-      s.forced = s.epoch - round_epoch0 >= P.force_epoch ? 1u : 0u;
-      job->stats.forced_launches += s.forced;
-      CK(cudaMemsetAsync(s.bits_cur, 0, 2 * (size_t)nwords * 4, st));
-      CK(cudaMemsetAsync(s.srch_cur, 0, nwords * 4, st));
-      CK(cudaMemsetAsync(s.counters + 4, 0, 4, st));
-      CK(cudaMemsetAsync(s.counters + 16, 0, 4, st));
-      cudaEventRecord(ev[6], st);
-      const u32 wg = (n_sched + BR_WALK_WARPS - 1) / BR_WALK_WARPS;
-      br_walk_dispatch(P, [&](auto g, auto m) { k_walk<decltype(g)::value, decltype(m)::value><<<wg, 32 * BR_WALK_WARPS, 0, st>>>(s); });
-      cudaEventRecord(ev[7], st);
-      walk_pending = true; ++job->stats.walk_launches; job->stats.launches += 6;
-      job->stats.walk_bytes += (u64)n_sched * ch;
-      CK(cudaMemcpyAsync((u32*)s.bits_prev, s.bits_latest, nwords * 4, cudaMemcpyDeviceToDevice, st));
-      if (!P.quick) {   // (quality 2..4 check every run instead of marking: br_verify_run)
-        CK(cudaMemsetAsync(s.cover_cur, 0, nwords * 4, st));
-        k_cover<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s);
-      }
-      k_commit<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s);
-      if (P.quick) k_verify<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s);
-      else {
-        k_snapshot_update<<<(u32)((nwords + 255) / 256), 256, 0, st>>>(s, storedS, cntS);
-        refresh_prefS();
-      }
-    }
-    cudaEventRecord(ev[2], st);
-#ifdef BR_DEBUG_KNOBS
-    if (trace) {   // the slowest chunk walks of the final state, and a per-megabyte profile
-      std::vector<BrBlockOut> hb2(nb);
-      cudaMemcpyAsync(hb2.data(), s.bout, nb * sizeof(BrBlockOut), cudaMemcpyDeviceToHost, st); cudaStreamSynchronize(st);
-      const u32 per = (1u << 20) >> P.chunk_bits;
-      for (u32 a = 0; a < nb; a += per) {
-        unsigned long long cyc = 0, se = 0, ro = 0; u32 mx = 0;
-        for (u32 k = a; k < a + per && k < nb; ++k) { cyc += hb2[k].dbg_kcycles; se += hb2[k].dbg_searches; ro += hb2[k].dbg_rows; if (hb2[k].dbg_kcycles > mx) mx = hb2[k].dbg_kcycles; }
-        fprintf(stderr, "MiB %4u: %7.2f Mcycles per chunk (max %7.2f)  searches/chunk %5llu rows/search %5.1f\n", a / per, cyc / 1024.0 / per, mx / 1024.0, se / per, se ? (double)ro / se : 0.0);
-      }
-    }
-#endif
-    // ---- entropy stage
-    std::vector<BrMetaBlock> hm(n_mbs);
-    CK(cudaMemcpyAsync(hm.data(), s.mbs, n_mbs * sizeof(BrMetaBlock), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    BrMbLayout L;
-    br_mb_layout(P, hm.data(), n_mbs, L);
-    const size_t C = total_cmds;
-    BrEnt e; memset(&e, 0, sizeof(e));
-    BrCmd* cmds_all; u64 *soff, *ooff; BrCopyDesc* desc; u32 *out, *res, *lit_ord, *cmd_pos, *dist_ord, *stmp, *code_base;
-    BrHTree* tree_pool;
-    auto carve2 = [&](BrCarve& B) {
-      e.scratch = B.take<u8>(L.scratch_bytes + 256); e.outbits = B.take<u32>(L.out_words + 64);
-      out = B.take<u32>(L.out_cap / 4 + 16); e.cmds = cmds_all = B.take<BrCmd>(C + 1);
-      e.scratch_off = soff = B.take<u64>(n_mbs); e.out_off = ooff = B.take<u64>(n_mbs);
-      desc = B.take<BrCopyDesc>(n_mbs); res = B.take<u32>(16);
-      e.lit_ord = lit_ord = B.take<u32>(C + 2); e.cmd_pos = cmd_pos = B.take<u32>(C + 2); e.dist_ord = dist_ord = B.take<u32>(C + 2);
-      e.cmd_len = B.take<u32>(C + 2); e.lit_bit_base = B.take<u32>(C + 2); e.cmd_mb = B.take<u32>(C + 2);
-      e.dist_sym = B.take<u16>(C + 2);
-      e.lit_pos = B.take<u32>((size_t)n + 2); e.lit_cmd = B.take<u32>((size_t)n + 2); e.lit_len = B.take<u32>((size_t)n + 2);
-      e.aux = B.take<BrMbAux>(n_mbs);
-      code_base = B.take<u32>(n_mbs + 1);
-      tree_pool = B.take<BrHTree>((size_t)((L.code_workers + 63) & ~63u) * BR_CODE_TREE_NODES);
-      stmp = B.take<u32>(scan_tmp_words((size_t)n + C + 8) * 2);
-    };
-    if (!br_carve(job->arena2, carve2)) return 0;
-    CK(cudaMemcpyAsync(soff, L.scratch_off.data(), n_mbs * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(ooff, L.out_off.data(), n_mbs * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(e.outbits, 0, (L.out_words + 64) * 4, st));
-    CK(cudaMemsetAsync(out, 0, L.out_cap + 64, st));
-    k_compact<<<(nb * 32 + 127) / 128, 128, 0, st>>>(s, cmds_all, s.block_mb);
-    cudaEventRecord(ev[8], st);
-    // E0: ordinals
-    k_cmd_scan_inputs<<<(u32)((C + 1 + 255) / 256), 256, 0, st>>>(cmds_all, (u32)C, lit_ord, cmd_pos, dist_ord);
-    scan_exclusive(lit_ord, (u32)C + 1, stmp, st);
-    scan_exclusive(cmd_pos, (u32)C + 1, stmp, st);
-    scan_exclusive(dist_ord, (u32)C + 1, stmp, st);
-    CK(cudaMemcpyAsync(hp + 24, lit_ord + C, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(hp + 25, dist_ord + C, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    e.total_cmds = (u32)C; e.total_lits = hp[24]; e.total_dist = hp[25];
-    if (e.total_lits > n) return 0;
-    const u32 grid_mbs = n_mbs < 65535u ? n_mbs : 65535u;
-    k_cmd_mb<<<dim3(64, grid_mbs), 256, 0, st>>>(s, e.cmd_mb, n_mbs);
-    k_expand<<<(u32)((C + 127) / 128 + 1), 128, 0, st>>>(e);
-    if (!launch_split(s, e, n_mbs, st)) return 0;
-    if (P.mb_kind) k_prep_flat<<<n_mbs, 64, 0, st>>>(s, e);   // qualities 2, 3: no block split, one code per category
-    else launch_codes(s, e, L, n_mbs, code_base, stmp, tree_pool, 0, st);
-    k_lit_bits<<<(e.total_lits + 1 + 255) / 256, 256, 0, st>>>(s, e);
-    k_cmd_bits<<<(u32)((C + 1 + 255) / 256), 256, 0, st>>>(s, e);
-    scan_exclusive(e.lit_len, e.total_lits + 1, stmp, st);
-    scan_exclusive(e.cmd_len, (u32)C + 1, stmp, st);
-    k_emit_cmd<<<(u32)((C + 255) / 256), 256, 0, st>>>(s, e);
-    if (e.total_lits) k_emit_lit<<<(e.total_lits + 255) / 256, 256, 0, st>>>(s, e);
-    cudaEventRecord(ev[9], st);
+    if (!stage_fixpoint(job, s, b, trace, &n_mbs, &total_cmds) || !stage_entropy(job, s, b, n_mbs, total_cmds)) return 0;
     cudaEventRecord(ev[3], st);
     ++job->stats.encode_launches; job->stats.launches += 28;
-    k_assemble_scan<<<1, 32, 0, st>>>(s, ooff, out, desc, res, plan.with_header, cut_kind, cut_end, stream_end);
-    CK(cudaMemcpyAsync(hp + 16, res, 16, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (hp[18]) {   // encode.c:604: a coded metablock is larger than its input -> it is stored raw (br_assemble_scan marked
-                    // it in force_unc) and the parse behind it is redone with the restored distance cache
-      if (rounds > (int)plan.max_rounds) return 0;
-      continue;
-    }
-    k_assemble_copy<<<dim3(64, grid_mbs), 256, 0, st>>>(s, desc, e.outbits, out, n_mbs);
-    final_out = (const u8*)out; final_size = ((u64)hp[17] << 32) | hp[16];
-    break;
+    bool redo;
+    if (!stage_assemble(job, s, b, plan.with_header, n_mbs, &redo, &final_out, &final_size)) return 0;
+    if (!redo) break;
+    if (rounds > (int)plan.max_rounds) return 0;
   }
   cudaEventRecord(ev[4], st);
   CK(cudaStreamSynchronize(st));
@@ -897,14 +919,14 @@ static int job_compress(BrJob* job, int quality, int lgwin, u32 size_hint, const
   cudaEventElapsedTime(&ms, ev[0], ev[4]); job->stats.ms_total = ms;
   cudaEventElapsedTime(&ms, ev[8], ev[9]); job->stats.ms_encode = ms;
   job->stats.total_cmds = total_cmds; job->stats.launches += 12;
-  job->stats.nblocks = nb; job->stats.n_metablocks = n_mbs; job->stats.rounds = (u32)rounds;
+  job->stats.nblocks = P.nblocks; job->stats.n_metablocks = n_mbs; job->stats.rounds = (u32)rounds;
   job->stats.out_bytes = final_size; job->stats.in_bytes = n;
   if (cuts && cuts->end_bit && ncuts && nstreams == 1) {
-    CK(cudaMemcpyAsync(cuts->end_bit, cut_end, ncuts * 8ull, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(cuts->end_bit, b.cut_end, ncuts * 8ull, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
   if (cuts && cuts->stream_end && nstreams > 1) {
-    CK(cudaMemcpyAsync(cuts->stream_end, stream_end, nstreams * 8ull, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(cuts->stream_end, b.stream_end, nstreams * 8ull, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
   *d_out = final_out; *out_size = final_size;
@@ -985,8 +1007,8 @@ extern "C" __attribute__((visibility("default"))) int br_debug_sort(int quality,
 }
 
 // Test hook (tests/test_search_probe.py): one match search per probe (br_probe.h), one warp each, from a state the caller
-// specifies.  The index (br_build_index), tagS (k_tags), the S-ordered snapshot (k_build_storedS and its prefix) and, at
-// qualities 2..4, the slot entry points (k_slot_pred) are built by the pipeline's own kernels.
+// specifies.  The index, tagS and, at qualities 2..4, the slot entry points are built by the pipeline's index stage
+// (stage_index, with tagS at every quality), the S-ordered snapshot by its snapshot stage (stage_snapshot).
 template <int F>
 __global__ void k_search_probe(BrStream s, u32* own, const u32* probes, u32 np, u32* res) {
   const u32 t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -1017,15 +1039,15 @@ extern "C" __attribute__((visibility("default"))) int br_debug_search(
   const size_t nsaw = P.quick ? ((size_t)n << P.qk_sweep_bits) + 16 : 16;
   BrStream s; memset(&s, 0, sizeof(s));
   s.P = P; s.nblk = nblk; s.bits_words = nwords;
-  BrIndexBufs b;
-  u8* data; u32 *snap, *own, *storedS, *prefS, *cntS, *scan_tmp2, *qpred, *probes, *res;
+  BrJobBufs b;
+  u8* data; u32 *snap, *own, *probes, *res;
   auto carve = [&](BrCarve& A) {
     s.data = data = A.take<u8>((size_t)n + 64); s.blk = A.take<BrBlk>(nblk); s.slot_blk = A.take<u32>(plan.slot_blk.size());
-    carve_index(A, P, b); carve_index_quick(A, P, b);
-    s.bits_latest = snap = A.take<u32>(nwords); own = A.take<u32>(nwords); s.storedS = storedS = A.take<u32>(nwords + 64);
-    s.prefS = prefS = A.take<u32>((size_t)n / 1024 + 8); cntS = A.take<u32>((size_t)n / 1024 + 8);
-    scan_tmp2 = A.take<u32>(scan_tmp_words((size_t)n / 1024 + 8));
-    s.qpred = qpred = A.take<u32>(nsaw); s.saw = A.take<u32>(nsaw);
+    carve_index(A, P, b.ix); carve_index_quick(A, P, b.ix);
+    s.bits_latest = snap = A.take<u32>(nwords); own = A.take<u32>(nwords); s.storedS = A.take<u32>(nwords + 64);
+    s.prefS = A.take<u32>((size_t)n / 1024 + 8); b.cntS = A.take<u32>((size_t)n / 1024 + 8);
+    b.scan_tmp2 = A.take<u32>(scan_tmp_words((size_t)n / 1024 + 8));
+    s.qpred = A.take<u32>(nsaw); s.saw = A.take<u32>(nsaw);
     probes = A.take<u32>((size_t)np * BR_PROBE_WORDS); res = A.take<u32>((size_t)np * BR_PROBE_WORDS * nvar);
   };
   auto probe = [&](auto g, int v) {
@@ -1033,7 +1055,7 @@ extern "C" __attribute__((visibility("default"))) int br_debug_search(
   };
   BrArena A;
   if (!br_carve(A, carve)) return 0;
-  s.S = b.S; s.rank = b.rank; s.seg = b.seg; s.skeys = b.K2; s.tagS = b.tagS;
+  s.S = b.ix.S; s.rank = b.ix.rank; s.seg = b.ix.seg; s.skeys = b.ix.K2; s.tagS = b.ix.tagS;
   br_bind_tables(s, T->blob, T->log2tab, T->log2tab_n);
   int ok = 0;
   if (cudaMemset(data, 0, (size_t)n + 64) != cudaSuccess || cudaMemcpy(data, h_in, n, cudaMemcpyHostToDevice) != cudaSuccess ||
@@ -1044,19 +1066,15 @@ extern "C" __attribute__((visibility("default"))) int br_debug_search(
       cudaMemcpy(own, h_own, (n + 31) / 32 * 4ull, cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemset(s.saw, 0xEE, nsaw * 4) != cudaSuccess ||
       cudaMemcpy(probes, h_probes, (size_t)np * BR_PROBE_WORDS * 4, cudaMemcpyHostToDevice) != cudaSuccess) goto done;
-  br_build_index(P, data, s.blk, nblk, b, 0);
-  if (P.quick) k_slot_pred<<<nblk, 256, 0>>>(s, qpred);
-  k_tags<<<(n + 255) / 256, 256>>>(data, b.S, n, b.tagS);
-  k_build_storedS<<<nsnap, 1024>>>(s, storedS, cntS);
-  if (cudaMemcpy(prefS, cntS, nsnap * 4ull, cudaMemcpyDeviceToDevice) != cudaSuccess) goto done;
-  scan_exclusive(prefS, nsnap, scan_tmp2, 0);
+  stage_index(s, b.ix, true, 0);
+  stage_snapshot(s, b.cntS, b.scan_tmp2, 0);
   br_walk_dispatch(P, [&](auto g, auto) { probe(g, 0); });
   if (nvar == 3) { probe(std::integral_constant<int, 1>(), 1); probe(std::integral_constant<int, 8>(), 2); }
   if (cudaDeviceSynchronize() != cudaSuccess ||
       cudaMemcpy(h_res, res, (size_t)np * BR_PROBE_WORDS * 4 * nvar, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
-  if (h_tagS && cudaMemcpy(h_tagS, b.tagS, 2ull * n, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
-  if (h_storedS && cudaMemcpy(h_storedS, storedS, (n + 31) / 32 * 4ull, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
-  if (h_prefS && cudaMemcpy(h_prefS, prefS, nsnap * 4ull, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  if (h_tagS && cudaMemcpy(h_tagS, b.ix.tagS, 2ull * n, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  if (h_storedS && cudaMemcpy(h_storedS, s.storedS, (n + 31) / 32 * 4ull, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+  if (h_prefS && cudaMemcpy(h_prefS, s.prefS, nsnap * 4ull, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
   ok = nvar;
 done:
   cudaGetLastError();
@@ -1064,7 +1082,7 @@ done:
   return ok;
 }
 
-// Test hook (tests/test_entropy_codes.py): E4 alone, by the pipeline's own launches (launch_codes), on n_mbs synthetic
+// Test hook (tests/test_entropy_codes.py): E4 alone by the pipeline's launch_codes and carve_entropy, on n_mbs synthetic
 // metablocks (br_codes_synth: counts, histos).  The scratch and the thread workers' tree pool start filled with a nonzero
 // pattern, as a reused arena leaves them.  code_ctas: CTAs of thread workers (0: the pipeline's count).  Per code, in code
 // order: H (the smoothed counts), depth, bits (256, 704 or 64 entries each).  offsets: per compressed metablock the bit
@@ -1080,15 +1098,12 @@ extern "C" __attribute__((visibility("default"))) int br_debug_codes(u32 n_mbs, 
   BrStream s; memset(&s, 0, sizeof(s));
   s.P.n = n_mbs * BR_SYNTH_MB_BYTES;
   br_bind_tables(s, T->blob, T->log2tab, T->log2tab_n);
-  BrEnt e; memset(&e, 0, sizeof(e));
   const u32 ctas = L.code_workers ? codes_ctas(L, code_ctas) : 0u;
-  u64 *soff, *ooff; u32 *code_base, *stmp; BrHTree* pool;
-  auto carve = [&](BrCarve& A) {
-    e.scratch = A.take<u8>(img.size()); e.outbits = A.take<u32>(L.out_words + 64);
-    e.scratch_off = soff = A.take<u64>(n_mbs); e.out_off = ooff = A.take<u64>(n_mbs);
-    e.aux = A.take<BrMbAux>(n_mbs); s.mbs = A.take<BrMetaBlock>(n_mbs);
-    code_base = A.take<u32>(n_mbs + 1); stmp = A.take<u32>(scan_tmp_words(n_mbs + 1) * 2);
-    pool = A.take<BrHTree>((size_t)ctas * 64 * BR_CODE_TREE_NODES + 1);
+  BrJobBufs b;
+  const BrEnt& e = b.e;
+  auto carve = [&](BrCarve& A) {   // (no commands and no input: n_mbs bytes size the scan of the code counts)
+    carve_entropy(A, L, n_mbs, 0, (size_t)ctas * 64, b);
+    s.mbs = A.take<BrMetaBlock>(n_mbs);
   };
   BrArena A;
   if (!br_carve(A, carve)) return 0;
@@ -1097,13 +1112,13 @@ extern "C" __attribute__((visibility("default"))) int br_debug_codes(u32 n_mbs, 
   std::vector<u8> sc;
   if (cudaMemcpy(e.scratch, img.data(), img.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemset(e.outbits, 0, (L.out_words + 64) * 4) != cudaSuccess ||
-      cudaMemcpy(soff, L.scratch_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(ooff, L.out_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy((u64*)e.scratch_off, L.scratch_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy((u64*)e.out_off, L.out_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy(e.aux, ha.data(), n_mbs * sizeof(BrMbAux), cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy((BrMetaBlock*)s.mbs, hm.data(), n_mbs * sizeof(BrMetaBlock), cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemset(pool, 0xA5, ((size_t)ctas * 64 * BR_CODE_TREE_NODES + 1) * sizeof(BrHTree)) != cudaSuccess) goto done;
-  launch_codes(s, e, L, n_mbs, code_base, stmp, pool, code_ctas, 0);
-  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(&total, code_base + n_mbs, 4, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
+      cudaMemset(b.tree_pool, 0xA5, (size_t)ctas * 64 * BR_CODE_TREE_NODES * sizeof(BrHTree)) != cudaSuccess) goto done;
+  launch_codes(s, e, L, n_mbs, b.code_base, b.stmp, b.tree_pool, code_ctas, 0);
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(&total, b.code_base + n_mbs, 4, cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
   sc.resize(img.size());
   if (cudaMemcpy(sc.data(), e.scratch, img.size(), cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
   for (u32 i = 0; i < n_mbs; ++i) {
@@ -1123,8 +1138,8 @@ done:
 }
 
 // Test hook (tests/test_entropy_split.py): E0..E4 on metablocks the caller describes (br_split_synth: n input bytes, ncmd
-// commands of 16 bytes, BR_SPLIT_MB_WORDS words per metablock), by the pipeline's own launches: the E0 scans, k_expand,
-// launch_split and launch_codes.  The scratch starts filled with a nonzero pattern, as a reused arena leaves it.  Writes
+// commands of 16 bytes, BR_SPLIT_MB_WORDS words per metablock), by the pipeline's launch_e01, launch_split and launch_codes
+// over its arena layout (carve_entropy).  The scratch starts with a nonzero pattern, as a reused arena leaves it.  Writes
 // the records of the compressed metablocks (br_split_record, br_split_record_bits) to out, at most out_cap words, and
 // returns the words they take (0: failure); no symbol is coded and nothing is assembled.
 extern "C" __attribute__((visibility("default"))) long br_debug_split(const u8* h_in, u32 n, const BrCmd* h_cmds, u32 ncmd,
@@ -1138,23 +1153,12 @@ extern "C" __attribute__((visibility("default"))) long br_debug_split(const u8* 
   BrDeviceTables* T = get_tables();
   if (!T) return 0;
   br_bind_tables(s, T->blob, T->log2tab, T->log2tab_n);
-  u32 total_lits = 0, total_dist = 0;
-  for (u32 i = 0; i < ncmd; ++i) {
-    total_lits += h_cmds[i].insert_len; total_dist += (h_cmds[i].copy_len & 0x1FFFFFF) && h_cmds[i].cmd_prefix >= 128;
-  }
-  BrEnt e; memset(&e, 0, sizeof(e));
-  e.total_cmds = ncmd; e.total_lits = total_lits; e.total_dist = total_dist;
-  u64 *soff, *ooff; u32 *lit_ord, *cmd_pos, *dist_ord, *code_base, *stmp; BrHTree* pool;
-  const size_t pool_nodes = (size_t)((L.code_workers + 63) & ~63u) * BR_CODE_TREE_NODES + 1;
+  const size_t workers = (L.code_workers + 63) & ~63u;
+  BrJobBufs b;
+  BrEnt& e = b.e;
   auto carve = [&](BrCarve& A) {
-    s.data = A.take<u8>((size_t)n + 64); e.cmds = A.take<BrCmd>(ncmd + 1);
-    e.lit_ord = lit_ord = A.take<u32>(ncmd + 2); e.cmd_pos = cmd_pos = A.take<u32>(ncmd + 2); e.dist_ord = dist_ord = A.take<u32>(ncmd + 2);
-    e.lit_pos = A.take<u32>(total_lits + 2); e.lit_cmd = A.take<u32>(total_lits + 2); e.dist_sym = A.take<u16>(ncmd + 2);
-    e.scratch = A.take<u8>(L.scratch_bytes + 256); e.outbits = A.take<u32>(L.out_words + 64);
-    e.scratch_off = soff = A.take<u64>(n_mbs); e.out_off = ooff = A.take<u64>(n_mbs);
-    e.aux = A.take<BrMbAux>(n_mbs); s.mbs = A.take<BrMetaBlock>(n_mbs);
-    code_base = A.take<u32>(n_mbs + 1); stmp = A.take<u32>(scan_tmp_words((size_t)n + ncmd + 8) * 2);
-    pool = A.take<BrHTree>(pool_nodes);
+    carve_entropy(A, L, n, ncmd, workers, b);
+    s.data = A.take<u8>((size_t)n + 64); s.mbs = A.take<BrMetaBlock>(n_mbs);
   };
   BrArena A;
   if (!br_carve(A, carve)) return 0;
@@ -1162,21 +1166,16 @@ extern "C" __attribute__((visibility("default"))) long br_debug_split(const u8* 
   std::vector<BrMbAux> ha(n_mbs);
   std::vector<std::vector<u32>> recs;
   std::vector<u8> img;
+  u32 totals[2];
   if (cudaMemset((u8*)s.data, 0, (size_t)n + 64) != cudaSuccess || cudaMemcpy((u8*)s.data, h_in, n, cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy((BrCmd*)e.cmds, h_cmds, ncmd * sizeof(BrCmd), cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemset(e.scratch, 0xA5, L.scratch_bytes + 256) != cudaSuccess ||
       cudaMemset(e.outbits, 0, (L.out_words + 64) * 4) != cudaSuccess ||
-      cudaMemcpy(soff, L.scratch_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(ooff, L.out_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy((u64*)e.scratch_off, L.scratch_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy((u64*)e.out_off, L.out_off.data(), n_mbs * 8ull, cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy((BrMetaBlock*)s.mbs, hm.data(), n_mbs * sizeof(BrMetaBlock), cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemset(pool, 0xA5, pool_nodes * sizeof(BrHTree)) != cudaSuccess) goto done;
-  // E0 and E1 as job_compress runs them
-  k_cmd_scan_inputs<<<(ncmd + 1 + 255) / 256, 256>>>(e.cmds, ncmd, lit_ord, cmd_pos, dist_ord);
-  scan_exclusive(lit_ord, ncmd + 1, stmp, 0);
-  scan_exclusive(cmd_pos, ncmd + 1, stmp, 0);
-  scan_exclusive(dist_ord, ncmd + 1, stmp, 0);
-  k_expand<<<(ncmd + 127) / 128 + 1, 128>>>(e);
-  if (!launch_split(s, e, n_mbs, 0) || cudaDeviceSynchronize() != cudaSuccess ||
+      cudaMemset(b.tree_pool, 0xA5, workers * BR_CODE_TREE_NODES * sizeof(BrHTree)) != cudaSuccess) goto done;
+  if (!launch_e01(s, e, ncmd, n_mbs, b.stmp, totals, 0) || !launch_split(s, e, n_mbs, 0) || cudaDeviceSynchronize() != cudaSuccess ||
       cudaMemcpy(ha.data(), e.aux, n_mbs * sizeof(BrMbAux), cudaMemcpyDeviceToHost) != cudaSuccess) goto done;
   for (u32 i = 0; i < n_mbs; ++i) {   // the splits and histograms before E4 smooths them
     if (!hm[i].compress) continue;
@@ -1185,7 +1184,7 @@ extern "C" __attribute__((visibility("default"))) long br_debug_split(const u8* 
     recs.emplace_back();
     br_split_record(hm[i], ha[i], img.data(), recs.back());
   }
-  launch_codes(s, e, L, n_mbs, code_base, stmp, pool, 0, 0);
+  launch_codes(s, e, L, n_mbs, b.code_base, b.stmp, b.tree_pool, 0, 0);
   if (cudaDeviceSynchronize() != cudaSuccess) goto done;
   for (u32 i = 0, r = 0; i < n_mbs; ++i) {
     if (!hm[i].compress) continue;

@@ -80,7 +80,14 @@ static inline u32 br_batch_chunk_bits(u32 n_total) { return n_total < (8u << 20)
 // last block carries is_last); otherwise the stream simply stops behind its last block.
 // kinds (nullable) = what each cut is: 1 FLUSH, 2 EMIT_METADATA, 3 = END OF A STREAM (a batch of independent streams laid
 // end to end, BrParams::multi): the block in front of the cut carries is_last, the blocks behind it belong to a new stream.
-// chunks == nullptr: only the block table (the CUDA pipeline fills the chunk table on the device, k_build_chunks).
+// chunks == nullptr: only the block table (the CUDA pipeline fills the chunk table on the device: k_build_chunks, by
+// br_chunk_in, the entry of chunk c of input block B, block index b, chunks of ch bytes).
+BR_HD BrBlockIn br_chunk_in(const BrBlk& B, u32 b, u32 c, u32 ch) {
+  BrBlockIn k; memset(&k, 0, sizeof(k));
+  k.pos = B.start + c * ch; k.end = k.pos + ch < B.end ? k.pos + ch : B.end; k.blk_start = B.start; k.blk_end = B.end;
+  k.first = c == 0; k.last = k.end == B.end; k.is_last = B.is_last; k.force_flush = B.force_flush; k.blk = b; k.base = B.base;
+  return k;
+}
 static inline void br_build_blocks(const BrParams& P, u32 n, const u32* cuts, u32 ncuts, bool is_final,
                                    std::vector<BrBlockIn>* chunks, std::vector<BrBlk>& blks, u32* nchunks_total = nullptr,
                                    const u32* kinds = nullptr) {
@@ -99,14 +106,7 @@ static inline void br_build_blocks(const BrParams& P, u32 n, const u32* cuts, u3
     B.force_flush = forced && !B.is_last ? 1u : 0u; B.changed_epoch = -1;
     B.first_chunk = total;
     B.nchunks = (u32)((bend - bstart + ch - 1) / ch);
-    if (chunks)
-      for (u64 c = bstart; c < bend; c += ch) {
-        BrBlockIn k; memset(&k, 0, sizeof(k));
-        k.pos = (u32)c; k.end = (u32)(c + ch < bend ? c + ch : bend); k.blk_start = (u32)bstart; k.blk_end = (u32)bend;
-        k.first = (c == bstart); k.last = (k.end == bend); k.is_last = B.is_last; k.force_flush = B.force_flush; k.blk = (u32)blks.size();
-        k.base = B.base;
-        chunks->push_back(k);
-      }
+    if (chunks) for (u32 c = 0; c < B.nchunks; ++c) chunks->push_back(br_chunk_in(B, (u32)blks.size(), c, ch));
     total += B.nchunks;
     blks.push_back(B);
     bstart = bend;

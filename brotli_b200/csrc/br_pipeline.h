@@ -5,7 +5,7 @@
 struct BrJob;
 struct BrJobStats {
   float ms_total, ms_index, ms_lz77, ms_entropy, ms_assemble;
-  float ms_walk, ms_encode;          // summed durations of the k_walk / k_encode_mb launches
+  float ms_walk, ms_encode;          // summed durations of the k_walk launches; E0..E7 of the entropy stage
   uint32_t walk_launches, encode_launches;
   uint64_t walk_bytes, total_cmds;   // input bytes walked (all launches), commands emitted
   uint32_t lz77_iterations, nblocks, n_metablocks, rounds, launches;

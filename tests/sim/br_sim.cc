@@ -381,13 +381,6 @@ extern "C" int sim_debug_sort(int q, int lgwin, const u8* in, u32 n, u32* S_out,
 }
 
 #ifdef BR_SIM_ENTROPY
-static void put_bits_host(std::vector<u8>& o, u64& bit, u32 n, u64 v) {
-  for (u32 i = 0; i < n; ++i, ++bit) {
-    if ((bit >> 3) >= o.size()) o.resize((bit >> 3) + 1, 0);
-    if ((v >> i) & 1) o[bit >> 3] |= (u8)(1u << (bit & 7));
-  }
-}
-
 // ---- the data-parallel entropy stage (br_entropy2.h), run element by element
 struct SimEnt {
   BrEnt e;
@@ -409,14 +402,14 @@ static void sim_split_mb(const BrStream& s, const BrEnt& e, const BrMetaBlock& m
                  br_mb2_lengths(sc, a, cat, nblk), BR_SPLIT_HIST(M, cat), smem);
   }
 }
-static void sim_entropy2(SimStream& m, SimEnt& E) {
-  BrStream& s = m.s;
-  u32 nm = s.counters[1], C = s.counters[2];
+// E0 and E1 (the pipeline's launch_e01) over the commands cmds[0 .. C) of the metablocks s.mbs[0 .. nm), with E.e wired
+// to E's arrays, those of the later stages sized too.  E.L: the metablocks' layout; the scratch starts filled with sc_fill.
+static void sim_e01(const BrStream& s, u32 nm, const BrCmd* cmds, u32 C, SimEnt& E, u8 sc_fill) {
   BrEnt& e = E.e;
-  e.cmds = m.cmds_all.data(); e.total_cmds = C;
+  e.cmds = cmds; e.total_cmds = C;
   E.lit_ord.assign(C + 1, 0); E.cmd_pos.assign(C + 1, 0); E.dist_ord.assign(C + 1, 0);
   for (u32 i = 0; i < C; ++i) {
-    u32 a, b, d; br_cmd_scan_inputs(e.cmds[i], &a, &b, &d);
+    u32 a, b, d; br_cmd_scan_inputs(cmds[i], &a, &b, &d);
     E.lit_ord[i + 1] = E.lit_ord[i] + a; E.cmd_pos[i + 1] = E.cmd_pos[i] + b; E.dist_ord[i + 1] = E.dist_ord[i] + d;
   }
   e.total_lits = E.lit_ord[C]; e.total_dist = E.dist_ord[C];
@@ -425,14 +418,20 @@ static void sim_entropy2(SimStream& m, SimEnt& E) {
   E.aux.assign(nm, BrMbAux());
   for (u32 i = 0; i < nm; ++i)
     for (u32 c = s.mbs[i].cmd_off; c < s.mbs[i].cmd_off + s.mbs[i].ncmd; ++c) E.cmd_mb[c] = i;
-  br_mb_layout(s.P, s.mbs, nm, E.L);
-  E.scratch.assign(E.L.scratch_bytes + 256, 0); E.outbits.assign(E.L.out_words + 64, 0);
+  E.scratch.assign(E.L.scratch_bytes + 256, sc_fill); E.outbits.assign(E.L.out_words + 64, 0);
   e.lit_ord = E.lit_ord.data(); e.cmd_pos = E.cmd_pos.data(); e.dist_ord = E.dist_ord.data();
   e.lit_pos = E.lit_pos.data(); e.lit_cmd = E.lit_cmd.data(); e.dist_sym = E.dist_sym.data();
   e.lit_len = E.lit_len.data(); e.cmd_len = E.cmd_len.data(); e.lit_bit_base = E.lit_bit_base.data();
   e.cmd_mb = E.cmd_mb.data(); e.aux = E.aux.data(); e.scratch = E.scratch.data(); e.scratch_off = E.L.scratch_off.data();
   e.outbits = E.outbits.data(); e.out_off = E.L.out_off.data();
   for (u32 c = 0; c < C; c += BR_WARP) br_expand_cmds(e, c);
+}
+static void sim_entropy2(SimStream& m, SimEnt& E) {
+  BrStream& s = m.s;
+  u32 nm = s.counters[1], C = s.counters[2];
+  BrEnt& e = E.e;
+  br_mb_layout(s.P, s.mbs, nm, E.L);
+  sim_e01(s, nm, m.cmds_all.data(), C, E, 0);
   std::vector<u32> smem(64 * 1024);
   for (u32 i = 0; i < nm; ++i) {
     const BrMetaBlock& mb = s.mbs[i];
@@ -484,7 +483,7 @@ static long sim_compress_impl(int q, int lgwin, u32 size_hint, const u8* in, u32
     if (getenv("BR_SIM_MBS"))   // metablock table (debugging against an instrumented reference)
       for (u32 i = 0; i < nm; ++i) fprintf(stderr, "SIMMB start %u bytes %u ncmd %u nlit %u last %u compress %u bits %u\n", s.mbs[i].start, s.mbs[i].end - s.mbs[i].start,
                                            s.mbs[i].ncmd, s.mbs[i].nlit, s.mbs[i].is_last, s.mbs[i].compress, s.mbs[i].out_bits);
-    // stream assembly: the shared scan (br_assemble.h), then the copies of k_assemble_copy
+    // stream assembly (br_assemble.h): the scan, then the copies word by word, as k_assemble_copy does them
     std::vector<u32> outw(E.L.out_cap / 4 + 16, 0);
     std::vector<BrCopyDesc> desc(nm + 1);
     std::vector<u64> cut_end((cuts ? cuts->n : 0) + 2, 0), stream_end(s.P.multi + 2, 0);
@@ -493,16 +492,8 @@ static long sim_compress_impl(int q, int lgwin, u32 size_hint, const u8* in, u32
                      cut_end.data(), stream_end.data());
     const bool redo = r4[2] != 0;
     if (!redo) {
-      for (u32 i = 0; i < nm; ++i) {
-        const BrCopyDesc& d = desc[i];
-        if (d.kind == 0) {
-          const u32* src = E.outbits.data() + d.src_off;
-          for (u32 b = 0; b < d.nbits; ++b) if ((src[b >> 5] >> (b & 31)) & 1) { const u64 db = d.dst_bit + b; outw[db >> 5] |= 1u << (db & 31); }
-        } else {
-          u8* ob = (u8*)outw.data() + (d.dst_bit >> 3);
-          memcpy(ob, in + d.src_off, d.nbits);
-        }
-      }
+      for (u32 i = 0; i < nm; ++i)
+        for (u32 w = 0, nw = br_copy_words(desc[i]); w < nw; ++w) br_copy_word(desc[i], w, E.outbits.data(), s.data, outw.data());
       const u64 total = ((u64)r4[1] << 32) | r4[0];
       res.assign((u8*)outw.data(), (u8*)outw.data() + total);
       if (cuts && cuts->end_bit) for (u32 i = 0; i < r4[3]; ++i) cuts->end_bit[i] = cut_end[i];
@@ -585,40 +576,25 @@ extern "C" long sim_debug_split(const u8* in, u32 n, const BrCmd* cmds, u32 ncmd
   if (n == 0 || n_mbs == 0 || quality < 4 || quality > 9) return 0;
   BrStream s; memset(&s, 0, sizeof(s));
   s.P.quality = quality; s.P.n = n; s.P.size_hint = size_hint; s.P.disable_ctx = disable_ctx ? 1u : 0u;
-  std::vector<BrMetaBlock> mbs; BrMbLayout L;
-  if (!br_split_synth(s.P, mbw, n_mbs, cmds, ncmd, mbs, L)) return 0;
+  std::vector<BrMetaBlock> mbs; SimEnt E;
+  if (!br_split_synth(s.P, mbw, n_mbs, cmds, ncmd, mbs, E.L)) return 0;
   std::vector<u8> data((size_t)n + 64, 0);
   memcpy(data.data(), in, n);
   s.data = data.data(); s.mbs = mbs.data();
   br_bind_tables(s, g_t.blob.data(), g_t.log2tab.data(), (u32)g_t.log2tab.size());
-  BrEnt e; memset(&e, 0, sizeof(e));
-  std::vector<u32> lit_ord(ncmd + 1, 0), cmd_pos(ncmd + 1, 0), dist_ord(ncmd + 1, 0);
-  for (u32 i = 0; i < ncmd; ++i) {
-    u32 a, b, d; br_cmd_scan_inputs(cmds[i], &a, &b, &d);
-    lit_ord[i + 1] = lit_ord[i] + a; cmd_pos[i + 1] = cmd_pos[i] + b; dist_ord[i + 1] = dist_ord[i] + d;
-  }
-  std::vector<u32> lit_pos(lit_ord[ncmd] + 1), lit_cmd(lit_ord[ncmd] + 1), outbits(L.out_words + 64, 0);
-  std::vector<u16> dist_sym(dist_ord[ncmd] + 1);
-  std::vector<BrMbAux> aux(n_mbs);
-  std::vector<u8> sc(L.scratch_bytes + 256, 0xA5);
-  e.cmds = cmds; e.total_cmds = ncmd; e.total_lits = lit_ord[ncmd]; e.total_dist = dist_ord[ncmd];
-  e.lit_ord = lit_ord.data(); e.cmd_pos = cmd_pos.data(); e.dist_ord = dist_ord.data();
-  e.lit_pos = lit_pos.data(); e.lit_cmd = lit_cmd.data(); e.dist_sym = dist_sym.data();
-  e.aux = aux.data(); e.scratch = sc.data(); e.scratch_off = L.scratch_off.data();
-  e.outbits = outbits.data(); e.out_off = L.out_off.data();
-  for (u32 c = 0; c < ncmd; c += BR_WARP) br_expand_cmds(e, c);
+  sim_e01(s, n_mbs, cmds, ncmd, E, 0xA5);
   std::vector<u32> smem(64 * 1024);
   std::vector<std::vector<u32>> recs;
   for (u32 i = 0; i < n_mbs; ++i) {
     if (!mbs[i].compress) continue;
-    u8* msc = sc.data() + L.scratch_off[i];
-    sim_split_mb(s, e, mbs[i], aux[i], msc, smem.data());
+    u8* msc = E.scratch.data() + E.L.scratch_off[i];
+    sim_split_mb(s, E.e, mbs[i], E.aux[i], msc, smem.data());
     recs.emplace_back();
-    br_split_record(mbs[i], aux[i], msc, recs.back());
-    u32* mout = outbits.data() + L.out_off[i];
-    br_prep_codes(s, mbs[i], aux[i], msc, mout);
+    br_split_record(mbs[i], E.aux[i], msc, recs.back());
+    u32* mout = E.outbits.data() + E.L.out_off[i];
+    br_prep_codes(s, mbs[i], E.aux[i], msc, mout);
     u32 nbits;
-    memcpy(&nbits, msc + br_split_code_end_off(mbs[i], aux[i]), 4);
+    memcpy(&nbits, msc + br_split_code_end_off(mbs[i], E.aux[i]), 4);
     br_split_record_bits(recs.back(), mout, nbits);
   }
   return (long)br_split_put(recs, out, out_cap);
