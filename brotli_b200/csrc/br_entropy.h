@@ -379,6 +379,19 @@ BR_DEV u32 br_static_ctx_map(int which, u32 ctx) {
 // the byte `back` positions in front of pos; zero in front of the stream's first byte (base)
 BR_DEV u8 br_data_or_zero(const BrStream& st, u32 pos, u32 back, u32 base) { return pos - base >= back ? st.data[pos - back] : 0; }
 
+// A CTA's threads (one in the CPU simulation) and its barrier.
+#if BR_GPU
+#define BR_CTA_TID ((u32)threadIdx.x)
+#define BR_CTA_N ((u32)blockDim.x)
+BR_DEV void br_cta_sync() { __syncthreads(); }
+BR_DEV u32 br_smem_add(u32* p, u32 v) { return atomicAdd(p, v); }
+#else
+#define BR_CTA_TID 0u
+#define BR_CTA_N 1u
+BR_DEV void br_cta_sync() {}
+BR_DEV u32 br_smem_add(u32* p, u32 v) { u32 o = *p; *p = o + v; return o; }
+#endif
+
 // encode.c:258 EstimateEntropy
 BR_DEV double br_estimate_entropy(const BrStream& st, const u32* pop, u32 size) {
   u32 total = 0; double result = 0;
@@ -389,58 +402,55 @@ BR_DEV double br_estimate_entropy(const BrStream& st, const u32* pop, u32 size) 
   }
   return br_dsub(br_dmul((double)total, br_fast_log2(st, total)), result);
 }
-// encode.c:424 DecideOverLiteralContextModeling; returns number of contexts (1, 2, 3 or 13).
-BR_DEV u32 br_decide_context_modeling(const BrStream& st, u32 start_pos, u32 length, u32* scratch /* >= 14*32 */) {
+// encode.c:424 DecideOverLiteralContextModeling; returns number of contexts (1, 2, 3 or 13).  Run by a whole CTA (one
+// thread in the CPU simulation), the strides spread over its threads; the counts are integers, so the order in which
+// the threads add them does not matter.  scratch: >= 14*32 words, shared memory in k_mb_setup.
+BR_DEV u32 br_decide_context_modeling(const BrStream& st, u32 start_pos, u32 length, u32* scratch) {
   const BrParams& P = st.P;
-  const int lane = br_lane();
+  const u32 tid = BR_CTA_TID, nt = BR_CTA_N;
   if (P.quality < 5 || length < 64) return 1;
   const u32 end_pos = start_pos + length;
   if (P.size_hint >= (1u << 20)) {
     u32* combined = scratch; u32* ctxh = scratch + 32;
-    for (u32 i = (u32)lane; i < 14 * 32; i += BR_WARP) scratch[i] = 0;
-    br_syncwarp();
+    for (u32 i = tid; i < 14 * 32; i += nt) scratch[i] = 0;
+    br_cta_sync();
     u32 nstrides = (length >= 64) ? (length - 64) / 4096 + 1 : 0;
-    for (u32 si = (u32)lane; si < nstrides; si += BR_WARP) {
+    for (u32 si = tid; si < nstrides; si += nt) {
       u32 sp = start_pos + si * 4096;
       u8 prev2 = st.data[sp], prev1 = st.data[sp + 1];
       for (u32 pos = sp + 2; pos < sp + 64; ++pos) {
         u8 lit = st.data[pos];
         u32 ctx = br_static_ctx_map(13, BR_CTX_UTF8(st, prev1, prev2));
-        br_atomic_add(combined + (lit >> 3), 1);
-        br_atomic_add(ctxh + (ctx << 5) + (lit >> 3), 1);
+        br_smem_add(combined + (lit >> 3), 1);
+        br_smem_add(ctxh + (ctx << 5) + (lit >> 3), 1);
         prev2 = prev1; prev1 = lit;
       }
     }
-#if BR_GPU
-    __threadfence_block();
-#endif
-    br_syncwarp();
+    br_cta_sync();
     u32 total = nstrides * 62;
     double e1 = br_estimate_entropy(st, combined, 32), e2 = 0;
     for (u32 i = 0; i < 13; ++i) e2 = br_dadd(e2, br_estimate_entropy(st, ctxh + (i << 5), 32));
     double e0 = br_ddiv(1.0, (double)total);
     e1 = br_dmul(e1, e0); e2 = br_dmul(e2, e0);
     if (!(e2 > 3.0 || br_dsub(e1, e2) < 0.2)) return 13;
+    br_cta_sync();   // (every thread has read `combined` before bigram, which overlaps it, is cleared)
   }
   {
     u32* bigram = scratch;
-    for (u32 i = (u32)lane; i < 16; i += BR_WARP) bigram[i] = 0;
-    br_syncwarp();
+    for (u32 i = tid; i < 16; i += nt) bigram[i] = 0;
+    br_cta_sync();
     u32 nstrides = (length - 64) / 4096 + 1;
-    for (u32 si = (u32)lane; si < nstrides; si += BR_WARP) {
+    for (u32 si = tid; si < nstrides; si += nt) {
       u32 sp = start_pos + si * 4096;
       const u8 lut[4] = {0, 0, 1, 2};
       u32 prev = lut[st.data[sp] >> 6] * 3u;
       for (u32 pos = sp + 1; pos < sp + 64; ++pos) {
         u8 lit = st.data[pos];
-        br_atomic_add(bigram + prev + lut[lit >> 6], 1);
+        br_smem_add(bigram + prev + lut[lit >> 6], 1);
         prev = lut[lit >> 6] * 3u;
       }
     }
-#if BR_GPU
-    __threadfence_block();
-#endif
-    br_syncwarp();
+    br_cta_sync();
     (void)end_pos;
     // encode.c:277 ChooseContextMap
     u32 mono[3] = {0, 0, 0}, two[6] = {0, 0, 0, 0, 0, 0};

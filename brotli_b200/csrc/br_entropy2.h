@@ -5,11 +5,12 @@
 //
 //   E0  prefix sums over commands      literal ordinal / input position / distance ordinal
 //   E1  br_expand_cmd                   literal ordinal -> input position, compact distance symbols
-//   E2  br_decide_context_modeling      (br_entropy.h; one warp per metablock)
-//   E3  br_split_cta                    greedy block split: the decision CHAIN of
-//                                       metablock_inc.h:86 is serial, but each link is executed by a
-//                                       whole CTA (histogram accumulation with shared-memory atomics,
-//                                       the 3 x contexts entropy sums on separate threads)
+//   E2  br_decide_context_modeling      (br_entropy.h; one CTA per metablock, shared-memory counts)
+//   E3  br_split_syms / br_split_cta    greedy block split: every symbol's histogram row as a u16
+//                                       array, then the decision CHAIN of metablock_inc.h:86, serial,
+//                                       each link executed by a whole CTA (16-byte symbol loads counted
+//                                       with shared-memory atomics, the 3 x contexts entropy sums on
+//                                       separate threads)
 //   E4  br_code_build / br_mb_header    smoothing + Huffman construction of every prefix code of the job
 //       / br_code_store                 in parallel, the header by one warp per metablock, then every
 //                                       code stored at its offset in parallel
@@ -18,18 +19,6 @@
 //   E6  br_emit_lit / br_emit_cmd       scatter of the code words with atomic OR
 #pragma once
 #include "br_entropy.h"
-
-#if BR_GPU
-#define BR_CTA_TID ((u32)threadIdx.x)
-#define BR_CTA_N ((u32)blockDim.x)
-BR_DEV void br_cta_sync() { __syncthreads(); }
-BR_DEV u32 br_smem_add(u32* p, u32 v) { return atomicAdd(p, v); }
-#else
-#define BR_CTA_TID 0u
-#define BR_CTA_N 1u
-BR_DEV void br_cta_sync() {}
-BR_DEV u32 br_smem_add(u32* p, u32 v) { u32 o = *p; *p = o + v; return o; }
-#endif
 
 // per-metablock results of the parallel stages
 struct BrMbAux {
@@ -105,7 +94,9 @@ struct BrEnt {
   const u32* dist_ord;     // [total_cmds + 1] exclusive scan of "has explicit distance"
   u32* lit_pos;            // [total_lits] input position of every literal
   u32* lit_cmd;            // [total_lits] command owning the literal
-  u16* dist_sym;           // [total_dist]
+  u16* dist_sym;           // [total_dist + 16]
+  u16* lit_sym;            // [total_lits + 16] E3's histogram row of every literal: context * 256 + byte (br_split_syms)
+  u16* cmd_sym;            // [total_cmds + 16] command prefix of every command
   u32* lit_len;            // [total_lits + 1] bit counts, then (in place) their exclusive scan
   u32* cmd_len;            // [total_cmds + 1] likewise for command + distance parts
   u32* lit_bit_base;       // [total_cmds] add the scanned lit_len of a literal to get its bit offset
@@ -191,9 +182,85 @@ BR_DEV void br_symbol_at(const BrStream& st, const BrEnt& e, const BrMetaBlock& 
     *sym = e.dist_sym[a.dist_base + o];
   }
 }
+// the histogram row of symbol `o` of category cat: context * 256 + byte for a literal, the symbol itself otherwise
+BR_DEV u16 br_split_row(const BrStream& st, const BrEnt& e, const BrMetaBlock& mb, const BrMbAux& a, int cat, u32 o) {
+  u32 sym, ctx;
+  br_symbol_at(st, e, mb, a, cat, o, &sym, &ctx);
+  return (u16)(ctx * 256 + sym);
+}
+// E3's symbols of compressed metablock mb as coalesced u16 arrays, element i of its literals and of its commands (E2 has
+// chosen a.which): their histogram rows.  Distances are dist_sym.
+BR_DEV void br_split_syms(const BrStream& st, const BrEnt& e, const BrMetaBlock& mb, const BrMbAux& a, u32 i) {
+  if (i < mb.nlit) e.lit_sym[a.lit_base + i] = br_split_row(st, e, mb, a, 0, i);
+  if (i < mb.ncmd) e.cmd_sym[mb.cmd_off + i] = br_split_row(st, e, mb, a, 1, i);
+}
+// 8 u16 from p (16-byte aligned) as 4 words
+BR_DEV void br_load_u16x8(const u16* p, u32 w[4]) {
+#if BR_GPU
+  const uint4 q = __ldg((const uint4*)p);
+  w[0] = q.x; w[1] = q.y; w[2] = q.z; w[3] = q.w;
+#else
+  memcpy(w, p, 16);
+#endif
+}
+// Counts the rows syms[b .. b + n) into cur.  Each thread reads whole 16-byte groups of 8 symbols, up to 4 groups before
+// it counts any, so that its loads are in flight together; of the groups at either end only what lies inside is counted
+// (the arrays are 16-byte aligned and padded by 16 symbols).  The counts are integers: their order does not matter.
+BR_DEV void br_split_count(const u16* syms, u32 b, u32 n, u32* cur) {
+  const u32 tid = BR_CTA_TID, nt = BR_CTA_N, end = b + n;
+  for (u32 g = (b & ~7u) + tid * 8; g < end; g += 32 * nt) {
+    u32 w[4][4] = {};
+#pragma unroll
+    for (u32 j = 0; j < 4; ++j)
+      if (g + j * 8 * nt < end) br_load_u16x8(syms + g + j * 8 * nt, w[j]);
+#pragma unroll
+    for (u32 j = 0; j < 4; ++j)
+#pragma unroll
+      for (u32 k = 0; k < 8; ++k) {
+        const u32 x = g + j * 8 * nt + k;
+        if (x >= b && x < end) br_smem_add(cur + ((w[j][k >> 1] >> (16 * (k & 1))) & 0xFFFFu), 1);
+      }
+  }
+}
+// Counts symbols [o, o + n) of category cat of metablock mb into cur.  On the GPU from the arrays br_split_syms has
+// written (k_split_syms); the CPU simulation, which has no such arrays, stages the same rows (br_split_row) in pieces that
+// keep the arrays' alignment and counts them with the same br_split_count.
+BR_DEV void br_split_take(const BrStream& st, const BrEnt& e, const BrMetaBlock& mb, const BrMbAux& a, int cat, u32 o,
+                          u32 n, u32* cur) {
+  const u32 base = cat == 0 ? a.lit_base : cat == 1 ? mb.cmd_off : a.dist_base;
+#if BR_GPU
+  br_split_count(cat == 0 ? e.lit_sym : cat == 1 ? e.cmd_sym : e.dist_sym, base + o, n, cur);
+#else
+  for (u32 k = 0; k < n;) {
+    u16 buf[1024 + 16] = {};
+    const u32 lead = (base + o + k) & 7u, m = br_min(n - k, 1024u);
+    for (u32 j = 0; j < m; ++j) buf[lead + j] = br_split_row(st, e, mb, a, cat, o + k + j);
+    br_split_count(buf, lead, m, cur);
+    k += m;
+  }
+#endif
+}
 // shared memory plan (u32 words): cur[nc*A] | comb[2*nc*A] | (8-aligned) terms[3*nc*(A|1)] doubles | ent[3*nc] | state
 BR_HD u32 br_split_smem_bytes(u32 A, u32 nc) {
   return (3 * nc * A) * 4 + 8 + (3 * nc * (A | 1) + 3 * nc) * 8 + (u32)sizeof(BrSplitState) + 16;
+}
+// -(sum of terms[0 .. A)) from 0.0, in index order, as the reference's BitsEntropy accumulates it, and *sum = the sum of
+// the counts p[0 .. A).  The zero terms (counts of 0 and 1) are subtracted too: r - (+0.0) is r bit for bit, -0.0
+// included, so the result is the reference's without a branch, and the loads of 8 entries go out before their
+// subtractions.
+BR_DEV double br_split_neg_sum(const double* terms, const u32* p, u32 A, u32* sum) {
+  double r = 0;
+  u32 s = 0, i = 0;
+  for (; i + 8 <= A; i += 8) {
+    double v[8];
+#pragma unroll
+    for (u32 k = 0; k < 8; ++k) { v[k] = terms[i + k]; s += p[i + k]; }
+#pragma unroll
+    for (u32 k = 0; k < 8; ++k) r = br_dsub(r, v[k]);
+  }
+  for (; i < A; ++i) { r = br_dsub(r, terms[i]); s += p[i]; }
+  *sum = s;
+  return r;
 }
 // One CTA = one (metablock, category).  H: [256/nc * nc][A] finished histograms (global).
 BR_DEV void br_split_cta(const BrStream& st, const BrEnt& e, const BrMetaBlock& mb, BrMbAux& a, int cat,
@@ -217,11 +284,7 @@ BR_DEV void br_split_cta(const BrStream& st, const BrEnt& e, const BrMetaBlock& 
     u32 take = 0;
     if (!final_call) {
       take = br_min(nsym - o, S->target - S->block_size);
-      for (u32 k = tid; k < take; k += nt) {
-        u32 sym, ctx;
-        br_symbol_at(st, e, mb, a, cat, o + k, &sym, &ctx);
-        br_smem_add(cur + ctx * A + sym, 1);
-      }
+      br_split_take(st, e, mb, a, cat, o, take, cur);
       o += take;
     }
     br_cta_sync();
@@ -239,8 +302,8 @@ BR_DEV void br_split_cta(const BrStream& st, const BrEnt& e, const BrMetaBlock& 
       for (u32 x = tid; x < nc * A; x += nt) { u32 t = x / A, i = x - t * A; u32 p = cur[x]; terms[t * AS + i] = p ? br_dmul((double)p, br_fast_log2(st, p)) : 0.0; }
       br_cta_sync();
       for (u32 t = tid; t < nc; t += nt) {
-        double r = 0; u32 sum = 0;
-        for (u32 i = 0; i < A; ++i) { double v = terms[t * AS + i]; sum += cur[t * A + i]; if (v != 0.0) r = br_dsub(r, v); }
+        u32 sum;
+        double r = br_split_neg_sum(terms + t * AS, cur + t * A, A, &sum);
         if (sum) r = br_dadd(r, br_dmul((double)sum, br_fast_log2(st, sum)));
         if (r < (double)sum) r = (double)sum;
         ent[t] = r;
@@ -268,8 +331,8 @@ BR_DEV void br_split_cta(const BrStream& st, const BrEnt& e, const BrMetaBlock& 
       br_cta_sync();
       for (u32 t = tid; t < 3 * nc; t += nt) {
         const u32* src = t < nc ? cur + t * A : comb + (t - nc) * A;
-        double r = 0; u32 sum = 0;
-        for (u32 i = 0; i < A; ++i) { double v = terms[t * AS + i]; sum += src[i]; if (v != 0.0) r = br_dsub(r, v); }
+        u32 sum;
+        double r = br_split_neg_sum(terms + t * AS, src, A, &sum);
         if (sum) r = br_dadd(r, br_dmul((double)sum, br_fast_log2(st, sum)));
         if (r < (double)sum) r = (double)sum;
         ent[t] = r;

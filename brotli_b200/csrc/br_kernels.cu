@@ -363,18 +363,28 @@ __global__ void k_expand(BrEnt e) {
   if (w * 32 >= e.total_cmds) return;
   br_expand_cmds(e, w * 32);
 }
-// one warp per metablock: literal context model + bookkeeping
-__global__ void __launch_bounds__(32) k_mb_setup(BrStream s, BrEnt e) {
+// one CTA per metablock: literal context model (its histograms in shared memory) + bookkeeping
+__global__ void __launch_bounds__(256) k_mb_setup(BrStream s, BrEnt e) {
+  __shared__ u32 hist[14 * 32];
   const u32 i = blockIdx.x;
   const BrMetaBlock mb = s.mbs[i];
   if (!mb.compress) return;
-  u8* sc = e.scratch + e.scratch_off[i];
-  BrMbMem* M = (BrMbMem*)sc;
-  u32 which = s.P.disable_ctx ? 1u : br_decide_context_modeling(s, mb.start, mb.end - mb.start, M->sc.rle_syms);
+  u32 which = s.P.disable_ctx ? 1u : br_decide_context_modeling(s, mb.start, mb.end - mb.start, hist);
   if (threadIdx.x == 0) {
     BrMbAux a;
     br_mb_aux_init(a, mb, e, which);
     e.aux[i] = a;
+  }
+}
+// E3's symbol arrays (br_split_syms) of every compressed metablock; grid.y = metablock (capped, see k_cmd_mb), grid.x
+// strides over its literals and commands
+__global__ void k_split_syms(BrStream s, BrEnt e, u32 n_mbs) {
+  for (u32 m = blockIdx.y; m < n_mbs; m += gridDim.y) {
+    const BrMetaBlock mb = s.mbs[m];
+    if (!mb.compress) continue;
+    const BrMbAux a = e.aux[m];
+    const u32 n = mb.nlit > mb.ncmd ? mb.nlit : mb.ncmd;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) br_split_syms(s, e, mb, a, i);
   }
 }
 __global__ void __launch_bounds__(256) k_split(BrStream s, BrEnt e) {
@@ -586,8 +596,9 @@ static void launch_codes(const BrStream& s, const BrEnt& e, const BrMbLayout& L,
 // E2 (the literal context decision and the metablock's BrMbAux) and, at qualities 4..9, E3 (the block splits and their
 // histograms): what launch_codes starts from.  Returns false on a CUDA error.
 static bool launch_split(const BrStream& s, const BrEnt& e, u32 n_mbs, cudaStream_t st) {
-  k_mb_setup<<<n_mbs, 32, 0, st>>>(s, e);
+  k_mb_setup<<<n_mbs, 256, 0, st>>>(s, e);
   if (s.P.mb_kind) return true;
+  k_split_syms<<<dim3(64, n_mbs < 65535u ? n_mbs : 65535u), 256, 0, st>>>(s, e, n_mbs);
   const size_t smem_split = br_split_smem_bytes(256, 13) > br_split_smem_bytes(704, 1) ? br_split_smem_bytes(256, 13) : br_split_smem_bytes(704, 1);
   CK(cudaFuncSetAttribute(k_split, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_split));
   k_split<<<dim3(n_mbs, 3), 256, smem_split, st>>>(s, e);
@@ -628,7 +639,7 @@ static void carve_entropy(BrCarve& B, const BrMbLayout& L, size_t n, size_t C, s
   b.desc = B.take<BrCopyDesc>(n_mbs); b.res = B.take<u32>(16);
   e.lit_ord = B.take<u32>(C + 2); e.cmd_pos = B.take<u32>(C + 2); e.dist_ord = B.take<u32>(C + 2);
   e.cmd_len = B.take<u32>(C + 2); e.lit_bit_base = B.take<u32>(C + 2); e.cmd_mb = B.take<u32>(C + 2);
-  e.dist_sym = B.take<u16>(C + 2);
+  e.dist_sym = B.take<u16>(C + 16); e.cmd_sym = B.take<u16>(C + 16); e.lit_sym = B.take<u16>(n + 16);
   e.lit_pos = B.take<u32>(n + 2); e.lit_cmd = B.take<u32>(n + 2); e.lit_len = B.take<u32>(n + 2);
   e.aux = B.take<BrMbAux>(n_mbs);
   b.code_base = B.take<u32>(n_mbs + 1);
