@@ -1,8 +1,5 @@
-// br_api.cc -- the BrotliEncoder* C ABI (include/brotli_b200.h) on top of the GPU pipeline.
-// Host-side mirror of the reference's stream driver, c/enc/encode.c: parameter handling
-// (:60 BrotliEncoderSetParameter, quality.h:59 SanitizeParams), the one-shot wrapper
-// (:1296 BrotliEncoderCompress with its :1264 MakeUncompressedStream fallback), and the
-// streaming state machine (:1634).  No compression happens on the host.
+// br_api.cc -- the BrotliEncoder* C ABI (include/brotli_b200.h) on top of the GPU pipeline: the per-thread device jobs,
+// the backend the host driver (br_driver.h) compresses through, and the entry points.  No compression happens on the host.
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -11,8 +8,10 @@
 #include <thread>
 #include <vector>
 #include "../../include/brotli_b200.h"
-#include "br_pipeline.h"
+#include "br_driver.h"
 #include "br_q1_host.h"
+
+using namespace br_driver;
 
 namespace {
 
@@ -43,6 +42,29 @@ bool ensure_q1() {
   tls.q1 = br_q1_job_create();
   return tls.q1 != nullptr;
 }
+bool ensure_job() {
+  if (tls.job) return true;
+  if (!have_device()) return false;
+  tls.job = br_job_create();
+  return tls.job != nullptr;
+}
+// Grow-only buffers of this thread: room for n bytes of device input, or of pinned staging.
+bool reserve_d_in(size_t n) {
+  if (tls.d_in_cap >= n) return true;
+  if (tls.d_in) cudaFree(tls.d_in);
+  tls.d_in = nullptr; tls.d_in_cap = 0;
+  if (cudaMalloc(&tls.d_in, n + 64) != cudaSuccess) { cudaGetLastError(); return false; }
+  tls.d_in_cap = n;
+  return true;
+}
+bool reserve_h_stage(size_t n) {
+  if (tls.h_stage_cap >= n) return true;
+  if (tls.h_stage) cudaFreeHost(tls.h_stage);
+  tls.h_stage = nullptr; tls.h_stage_cap = 0;
+  if (cudaMallocHost(&tls.h_stage, n + 64) != cudaSuccess) { cudaGetLastError(); return false; }
+  tls.h_stage_cap = n;
+  return true;
+}
 void record_q1_stats() {
   const BrQ1Stats* s = br_q1_job_stats(tls.q1);
   double* o = tls.last_q1;
@@ -50,20 +72,6 @@ void record_q1_stats() {
   o[6] = (double)s->streams; o[7] = (double)s->fragments; o[8] = (double)s->blocks; o[9] = (double)s->in_bytes;
   o[10] = (double)s->out_bytes; o[11] = (double)s->launches;
 }
-
-bool ensure_job() {
-  if (tls.job) return true;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    static bool warned = false;
-    if (!warned) { warned = true; fprintf(stderr, "brotli_b200: no CUDA device; this library has no CPU path\n"); }
-    return false;
-  }
-  tls.job = br_job_create();
-  return tls.job != nullptr;
-}
-
 void record_stats() {
   const BrJobStats* s = br_job_stats(tls.job);
   tls.last[0] = s->ms_total; tls.last[1] = s->ms_index; tls.last[2] = s->ms_lz77; tls.last[3] = s->ms_entropy;
@@ -73,66 +81,15 @@ void record_stats() {
   tls.last[13] = s->encode_launches; tls.last[14] = (double)s->walk_bytes; tls.last[15] = (double)s->total_cmds;
 }
 
-struct Params {
-  int mode = BROTLI_MODE_GENERIC, quality = 11, lgwin = 22, lgblock = 0;
-  uint32_t size_hint = 0, disable_ctx = 0, large_window = 0, npostfix = 0, ndirect = 0, stream_offset = 0,
-           base64 = 0;
-};
-// What the pipeline implements; everything else must fail rather than emit different bytes.
-bool supported(Params p) {
-  if (p.quality > 11) p.quality = 11;          // quality.h:60 SanitizeParams
-  if (p.quality < 0) p.quality = 0;
-  if (p.quality <= 2) p.large_window = 0;      // quality.h:63: no large window with the static entropy codes; lgwin clamps to 24
-  if (p.lgwin < 10) p.lgwin = 10;
-  if (p.lgwin > 24 && !p.large_window) p.lgwin = 24;
-  if (p.quality < 1 || p.quality > 9) return false;   /* quality 0: one-pass fragment coder; 10, 11: Zopfli path */
-  if (p.quality <= 4 ? p.lgwin > 24 : (p.lgwin < 17 || p.lgwin > 24)) return false;   /* quality 1..4: any regular window */
-  if (p.large_window || p.npostfix || p.ndirect || p.base64) return false;
-  if (p.stream_offset && p.quality < 5) return false;   /* STREAM_OFFSET: quality 5..9 only */
-  /* LGBLOCK and DISABLE_LITERAL_CONTEXT_MODELING are honoured at quality 5..9; at quality 1 the reference ignores both
-     (quality.h:79: lgblock = lgwin; no context modeling in the fragment coder) */
-  if (p.mode == BROTLI_MODE_FONT) return false;
-  return true;
-}
-
-// c/enc/encode.c:1264 MakeUncompressedStream
-size_t make_uncompressed_stream(const uint8_t* input, size_t input_size, uint8_t* output) {
-  size_t size = input_size, result = 0, offset = 0;
-  if (input_size == 0) { output[0] = 6; return 1; }
-  output[result++] = 0x21;
-  output[result++] = 0x03;
-  while (size > 0) {
-    uint32_t nibbles = 0, chunk, bits;
-    chunk = size > (1u << 24) ? (1u << 24) : (uint32_t)size;
-    if (chunk > (1u << 16)) nibbles = chunk > (1u << 20) ? 2 : 1;
-    bits = (nibbles << 1) | ((chunk - 1) << 3) | (1u << (19 + 4 * nibbles));
-    output[result++] = (uint8_t)bits;
-    output[result++] = (uint8_t)(bits >> 8);
-    output[result++] = (uint8_t)(bits >> 16);
-    if (nibbles == 2) output[result++] = (uint8_t)(bits >> 24);
-    memcpy(&output[result], &input[offset], chunk);
-    result += chunk; offset += chunk; size -= chunk;
-  }
-  output[result++] = 3;
-  return result;
-}
-
-// host buffer -> device -> pipeline -> host vector / buffer.  Returns 0 on failure.
-int compress_host(const Params& p, uint32_t size_hint, const uint8_t* in, size_t n, uint8_t* out, size_t out_cap,
-                  size_t* out_n, std::vector<uint8_t>* out_vec, const BrCuts* cuts = nullptr) {
+// The driver's backend on the device (Backend::compress): host buffer -> device -> pipeline -> host vector / buffer.
+int compress_host(const Params& p, uint32_t size_hint, const uint8_t* in, size_t n, const BrCuts* cuts, uint8_t* out, size_t out_cap,
+                  size_t* out_n, std::vector<uint8_t>* out_vec) {
   if (!supported(p) || n == 0 || n > (1u << 30)) return 0;
-  if (!ensure_job()) return 0;
-  if (tls.d_in_cap < n) {
-    if (tls.d_in) cudaFree(tls.d_in);
-    tls.d_in = nullptr; tls.d_in_cap = 0;
-    if (cudaMalloc(&tls.d_in, n + 64) != cudaSuccess) { cudaGetLastError(); return 0; }
-    tls.d_in_cap = n;
-  }
+  if (!ensure_job() || !reserve_d_in(n)) return 0;
   cudaStream_t st = (cudaStream_t)br_job_stream(tls.job);
   if (cudaMemcpyAsync(tls.d_in, in, n, cudaMemcpyHostToDevice, st) != cudaSuccess) return 0;
   const uint8_t* d_out = nullptr; size_t sz = 0;
-  int q = p.quality, w = p.lgwin > 24 ? 24 : p.lgwin < 10 ? 10 : p.lgwin;   /* quality.h:60 SanitizeParams */
-  if (!br_job_compress_device(tls.job, q, w, size_hint, tls.d_in, (uint32_t)n, &d_out, &sz, cuts)) return 0;
+  if (!br_job_compress_device(tls.job, p.quality, window_of(p), size_hint, tls.d_in, (uint32_t)n, &d_out, &sz, cuts)) return 0;
   record_stats();
   if (out_vec) { out_vec->resize(sz); out = out_vec->data(); out_cap = sz; }
   if (sz > out_cap) { *out_n = sz; return 2; }   /* compressed, but the caller's buffer is too small (encode.c:1336: "not finished") */
@@ -142,98 +99,23 @@ int compress_host(const Params& p, uint32_t size_hint, const uint8_t* in, size_t
   return 1;
 }
 
-// Quality 1 (two-pass fragment coder, br_q1.cu): one segment of one stream = a batch of one.  `calls`: sizes of the
-// CompressStream calls that delivered the input (nullptr: a single call).
-int compress_host_q1(const Params& p0, const uint8_t* in, size_t n, const std::vector<size_t>* calls,
-                     std::vector<uint8_t>* out_vec, int with_header = 1, int end_op = 2, uint32_t start_bits = 0, uint32_t* end_bit = nullptr) {
-  Params p = p0;
-  if (p.lgwin < 10) p.lgwin = 10;      // quality.h:60 SanitizeParams
-  if (p.lgwin > 24) p.lgwin = 24;
+// Quality 1 (two-pass fragment coder, br_q1.cu): one segment of one stream = a batch of one.
+int device_q1_segment(int lgwin, const uint8_t* in, size_t n, const std::vector<size_t>& calls, int with_header, int end_op,
+                      uint32_t start_bits, uint32_t* end_bit, std::vector<uint8_t>& out) {
   if (!ensure_q1() || n > (1u << 28)) return 0;
-  size_t cap = n + 16;
-  { size_t lim = (size_t)1 << p.lgwin, nc = calls ? calls->size() : 1; cap += 12 * (n / lim + nc + 2); }
-  out_vec->resize(cap);
+  const size_t cap = n + 16 + 12 * (n / ((size_t)1 << lgwin) + calls.size() + 2);
+  out.resize(cap);
   const uint8_t* ins[1] = {in}; size_t in_n[1] = {n};
-  const size_t* cl[1] = {calls ? calls->data() : nullptr}; size_t ncl[1] = {calls ? calls->size() : 0};
-  uint8_t* outs[1] = {out_vec->data()}; size_t out_n[1] = {cap}; int ok[1] = {0};
-  uint32_t sb[1] = {start_bits}, eb[1] = {0};
-  if (!br_q1_compress_batch(tls.q1, p.lgwin, 1, ins, in_n, calls ? cl : nullptr, calls ? ncl : nullptr, nullptr, outs, out_n, ok, 1,
-                            with_header, end_op, sb, eb))
+  const size_t* cl[1] = {calls.data()}; size_t ncl[1] = {calls.size()};
+  uint8_t* outs[1] = {out.data()}; size_t out_n[1] = {cap}; int ok[1] = {0};
+  if (!br_q1_compress_batch(tls.q1, lgwin, 1, ins, in_n, cl, ncl, nullptr, outs, out_n, ok, 1, with_header, end_op, &start_bits, end_bit))
     return 0;
   record_q1_stats();
-  out_vec->resize(out_n[0]);
-  if (end_bit) *end_bit = eb[0];
+  out.resize(out_n[0]);
   return 1;
 }
+const Backend kDevice = {compress_host, device_q1_segment};
 
-// What a quality-1 stream carries from one device segment to the next (encode.c:1445 last_bytes_ / last_bytes_bits_):
-// the bits of its last, incomplete byte, and whether the window bits went out.
-struct Q1Tail { uint32_t bits = 0; uint8_t byte = 0; bool header_done = false; };
-// One device segment holds at most this much input (bit offsets inside a segment are 32-bit); a stream is any number of them.
-static const size_t kQ1SegmentBytes = (size_t)1 << 27;
-
-template <class Vec>
-int q1_segment(const Params& p, const uint8_t* in, size_t n, const std::vector<size_t>& calls, int end_op, Q1Tail& t, Vec& out) {
-  const int with_header = !t.header_done;
-  if (n == 0) {
-    /* nothing to parse: window bits (encode.c:1006), ISLAST + ISEMPTY (compress_fragment_two_pass.c:641) or the
-       padding block of a FLUSH (encode.c:1356) behind the pending bits */
-    uint32_t acc = t.byte & ((1u << t.bits) - 1u), nb = t.bits;
-    if (with_header) {
-      int lgwin = p.lgwin > 24 ? 24 : p.lgwin;
-      if (lgwin < 18) lgwin = 18;      /* encode.c:673 */
-      acc |= (uint32_t)(((lgwin - 17) << 1) | 1) << nb; nb += 4;
-    }
-    if (end_op == 2) { acc |= 3u << nb; nb = (nb + 2 + 7) & ~7u; }
-    else if (end_op == 1 && (nb & 7)) { acc |= 6u << nb; nb = (nb + 6 + 7) & ~7u; }
-    while (nb >= 8) { out.push_back((uint8_t)acc); acc >>= 8; nb -= 8; }
-    t.bits = nb; t.byte = (uint8_t)acc;
-  } else {
-    std::vector<uint8_t> seg; uint32_t end_bit = 0;
-    if (!compress_host_q1(p, in, n, &calls, &seg, with_header, end_op, t.bits, &end_bit) || seg.empty()) return 0;
-    if (t.bits) seg[0] |= (uint8_t)(t.byte & ((1u << t.bits) - 1u));
-    t.bits = 0; t.byte = 0;
-    if (end_op == 0 && (end_bit & 7)) { t.bits = end_bit & 7; t.byte = seg.back(); seg.pop_back(); }
-    out.insert(out.end(), seg.begin(), seg.end());
-  }
-  t.header_done = true;
-  return 1;
-}
-
-// [in, in+n) as delivered by `calls` (nullptr: one call), through the device in segments of at most kQ1SegmentBytes.  A call
-// that straddles a segment is split at a multiple of the fragment size (1 << lgwin), which leaves the reference's fragments
-// (encode.c:1425) as they were.  Complete bytes are appended to `out`; end_op as in br_q1_host.h.
-template <class Vec>
-int q1_run(const Params& p, const uint8_t* in, size_t n, const size_t* calls, size_t ncalls, int end_op, Q1Tail& t, Vec& out) {
-  int lgwin = p.lgwin < 10 ? 10 : p.lgwin > 24 ? 24 : p.lgwin;
-  const size_t limit = (size_t)1 << lgwin;
-  if (!calls) { calls = &n; ncalls = 1; }
-  size_t ci = 0, rem = ncalls ? calls[0] : 0, pos = 0;
-  for (;;) {
-    std::vector<size_t> sc; size_t seg_n = 0;
-    while (ci < ncalls) {
-      const size_t room = kQ1SegmentBytes - seg_n;
-      if (rem <= room) { sc.push_back(rem); seg_n += rem; ++ci; rem = ci < ncalls ? calls[ci] : 0; continue; }
-      const size_t part = room / limit * limit;
-      if (part) { sc.push_back(part); seg_n += part; rem -= part; }
-      break;
-    }
-    const bool last = ci >= ncalls;
-    if (!q1_segment(p, in + pos, seg_n, sc, last ? end_op : 0, t, out)) return 0;
-    pos += seg_n;
-    if (last) return pos == n;
-  }
-}
-
-// Quality 5..9, streams shorter than 1 MiB: a group of them is ONE device job (the streams laid end to end, cuts of kind 3
-// in br_pipeline.h), so the launches, the fixpoint's host round trips and the copies are paid once per group instead of
-// once per stream.  idx: the streams of the group; encoded_sizes: capacity in, size out (0 = failed).  What
-// BrotliEncoderCompress adds around the encoder (encode.c:1345 raw-stream rule) is applied per stream.  Returns the
-// number of streams compressed.
-static const size_t kBatchGroupBytes = (size_t)128 << 20;
-// ... and at most this many streams: every metablock owns ~1.9 MB of scratch in the entropy stage (histograms for up to 256
-// block types per category, br_entropy.h BrMbMem), and a stream is at least one metablock
-static const size_t kBatchGroupStreams = 8192;
 template <class F> void batch_threads(int threads, size_t count, F f) {
   if (threads <= 1 || count < 64) { f(0, count); return; }
   std::vector<std::thread> th;
@@ -243,53 +125,40 @@ template <class F> void batch_threads(int threads, size_t count, F f) {
   }
   for (auto& t : th) t.join();
 }
-size_t compress_stream_group(int quality, int lgwin, const std::vector<size_t>& idx, const uint8_t* const* inputs,
+// One group of br_driver::plan_groups as one device job, through the pinned staging area: one upload, one download, and
+// BrotliEncoderCompress's raw-stream rule per stream.  idx: the streams of the group; encoded_sizes: capacity in, size
+// out (0 = failed).  Returns the number of streams compressed.
+size_t compress_stream_group(const Params& p, const std::vector<size_t>& idx, const uint8_t* const* inputs,
                              const size_t* input_sizes, uint8_t* const* outputs, size_t* encoded_sizes, int threads) {
   const size_t k = idx.size();
   auto fail_all = [&]() { for (size_t i : idx) encoded_sizes[i] = 0; return (size_t)0; };
   if (!ensure_job()) return fail_all();
-  std::vector<uint64_t> off(k + 1, 0);
-  uint32_t hint = 0;
-  for (size_t j = 0; j < k; ++j) { off[j + 1] = off[j] + input_sizes[idx[j]]; if (input_sizes[idx[j]] > hint) hint = (uint32_t)input_sizes[idx[j]]; }
-  const size_t n = off[k];
+  GroupCuts g(input_sizes, idx.data(), k);
+  const size_t n = g.n;
   const size_t out_bound = n + (n >> 3) + 4096 + 64 * k;
-  const size_t stage = n > out_bound ? n : out_bound;
-  if (tls.h_stage_cap < stage) {
-    if (tls.h_stage) cudaFreeHost(tls.h_stage);
-    tls.h_stage = nullptr; tls.h_stage_cap = 0;
-    if (cudaMallocHost(&tls.h_stage, stage + 64) != cudaSuccess) { cudaGetLastError(); return fail_all(); }
-    tls.h_stage_cap = stage;
-  }
-  if (tls.d_in_cap < n) {
-    if (tls.d_in) cudaFree(tls.d_in);
-    tls.d_in = nullptr; tls.d_in_cap = 0;
-    if (cudaMalloc(&tls.d_in, n + 64) != cudaSuccess) { cudaGetLastError(); return fail_all(); }
-    tls.d_in_cap = n;
-  }
+  if (!reserve_h_stage(n > out_bound ? n : out_bound) || !reserve_d_in(n)) return fail_all();
   uint8_t* hs = tls.h_stage;
-  batch_threads(threads, k, [&](size_t a, size_t b) { for (size_t j = a; j < b; ++j) memcpy(hs + off[j], inputs[idx[j]], input_sizes[idx[j]]); });
+  batch_threads(threads, k, [&](size_t a, size_t b) {
+    for (size_t j = a; j < b; ++j) memcpy(hs + (j ? g.pos[j - 1] : 0), inputs[idx[j]], input_sizes[idx[j]]);
+  });
   cudaStream_t st = (cudaStream_t)br_job_stream(tls.job);
   if (cudaMemcpyAsync(tls.d_in, hs, n, cudaMemcpyHostToDevice, st) != cudaSuccess) return fail_all();
-  std::vector<uint32_t> pos(k, 0), kind(k, 3);
-  for (size_t j = 0; j + 1 < k; ++j) pos[j] = (uint32_t)off[j + 1];
-  std::vector<uint64_t> ends(k + 1, 0);
-  BrCuts c; memset(&c, 0, sizeof(c));
-  c.pos = pos.data(); c.kind = kind.data(); c.n = (uint32_t)(k - 1); c.is_final = 1; c.with_header = 1; c.stream_end = ends.data();
   const uint8_t* d_out = nullptr; size_t sz = 0;
-  int w = lgwin > 24 ? 24 : lgwin < 10 ? 10 : lgwin;   /* quality.h:60 SanitizeParams */
-  if (!br_job_compress_device(tls.job, quality, w, hint, tls.d_in, (uint32_t)n, &d_out, &sz, k > 1 ? &c : nullptr)) return fail_all();
+  if (!br_job_compress_device(tls.job, p.quality, window_of(p), g.hint, tls.d_in, (uint32_t)n, &d_out, &sz, k > 1 ? &g.c : nullptr))
+    return fail_all();
   record_stats();
-  if (k == 1) ends[0] = sz;
-  if (sz > tls.h_stage_cap || ends[k - 1] != sz) return fail_all();
+  if (k == 1) g.ends[0] = sz;
+  if (sz > tls.h_stage_cap || g.ends[k - 1] != sz) return fail_all();
   if (cudaMemcpyAsync(hs, d_out, sz, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) return fail_all();
   std::vector<uint8_t> good(k, 0);
   batch_threads(threads, k, [&](size_t a, size_t b) {
     for (size_t j = a; j < b; ++j) {
-      const size_t i = idx[j], from = j ? (size_t)ends[j - 1] : 0, got = (size_t)ends[j] - from, cap = encoded_sizes[i];
-      const size_t bound = BrotliEncoderMaxCompressedSize(input_sizes[i]);
-      if (got <= cap && got <= bound) { memcpy(outputs[i], hs + from, got); encoded_sizes[i] = got; good[j] = 1; }
-      else if (cap >= bound) { encoded_sizes[i] = make_uncompressed_stream(inputs[i], input_sizes[i], outputs[i]); good[j] = 1; }   /* encode.c:1345 */
-      else encoded_sizes[i] = 0;
+      const size_t i = idx[j], from = j ? (size_t)g.ends[j - 1] : 0, got = (size_t)g.ends[j] - from;
+      switch (fit_stream(got, encoded_sizes[i], input_sizes[i])) {
+        case kKeep: memcpy(outputs[i], hs + from, got); encoded_sizes[i] = got; good[j] = 1; break;
+        case kRaw: encoded_sizes[i] = make_uncompressed_stream(inputs[i], input_sizes[i], outputs[i]); good[j] = 1; break;
+        default: encoded_sizes[i] = 0;
+      }
     }
   });
   size_t ok = 0;
@@ -299,139 +168,12 @@ size_t compress_stream_group(int quality, int lgwin, const std::vector<size_t>& 
 
 }  // namespace
 
-// Buffers of an encoder instance come from the caller's allocator pair when one was given (encode.h:295-306).
-template <class T> struct BrAlloc {
-  typedef T value_type;
-  brotli_alloc_func af = nullptr; brotli_free_func ff = nullptr; void* opaque = nullptr;
-  BrAlloc() {}
-  BrAlloc(brotli_alloc_func a, brotli_free_func f, void* o) : af(a), ff(f), opaque(o) {}
-  template <class U> BrAlloc(const BrAlloc<U>& o) : af(o.af), ff(o.ff), opaque(o.opaque) {}
-  T* allocate(size_t n) {
-    void* p = af ? af(opaque, n * sizeof(T)) : malloc(n * sizeof(T));
-    if (!p) throw std::bad_alloc();
-    return (T*)p;
-  }
-  void deallocate(T* p, size_t) { if (ff) ff(opaque, p); else free(p); }
-  template <class U> bool operator==(const BrAlloc<U>& o) const { return af == o.af && ff == o.ff && opaque == o.opaque; }
-  template <class U> bool operator!=(const BrAlloc<U>& o) const { return !(*this == o); }
-};
-typedef std::vector<uint8_t, BrAlloc<uint8_t>> ByteVec;
-
-// A FLUSH (kind 1) or EMIT_METADATA (kind 2) operation at input position pos (quality 5..9).
-struct StreamEvent { uint32_t pos; int kind; std::vector<uint8_t> meta; };
-
 struct BrotliEncoderStateStruct {
   brotli_alloc_func alloc_func; brotli_free_func free_func; void* opaque;
-  Params params;
-  bool initialized = false, finished = false, compressed = false, hint_fixed = false;
-  Q1Tail q1_tail;                // quality 1: pending bits between device segments, window bits sent
-  bool flint_done = false;       // STREAM_OFFSET: the cut behind the first two bytes has been recorded
-  ByteVec input, output;
-  std::vector<size_t> calls;     // quality 1: bytes brought by each CompressStream call (encode.c:1425 cuts fragments per call)
-  std::vector<StreamEvent> events;   // quality 5..9: the FLUSH / EMIT_METADATA operations so far
-  size_t wire_sent = 0;          // quality 5..9: bytes of the stream already handed to `output`
-  size_t out_pos = 0;
-  uint64_t total_out = 0;
+  Stream s;
   BrotliEncoderStateStruct(brotli_alloc_func a, brotli_free_func f, void* o)
-      : alloc_func(a), free_func(f), opaque(o), input(BrAlloc<uint8_t>(a, f, o)), output(BrAlloc<uint8_t>(a, f, o)) {}
+      : alloc_func(a), free_func(f), opaque(o), s(BrAlloc<uint8_t>(a, f, o)) {}
 };
-
-namespace {
-// LSB-first bit writer over a byte vector (c/enc/write_bits.h:33)
-struct BitOut {
-  std::vector<uint8_t>& v; uint32_t pb;   // pb: bits used in the last byte (0 = byte aligned)
-  void put(uint32_t n, uint64_t bits) {
-    for (uint32_t i = 0; i < n; ++i) {
-      if (pb == 0) v.push_back(0);
-      if ((bits >> i) & 1) v.back() |= (uint8_t)(1u << pb);
-      pb = (pb + 1) & 7;
-    }
-  }
-  void align() { pb = 0; }
-};
-// encode.c:1228 WriteMetadataHeader + the body (encode.c:1584)
-void put_metadata(BitOut& w, const std::vector<uint8_t>& meta) {
-  const size_t size = meta.size();
-  w.put(1, 0); w.put(2, 3); w.put(1, 0);
-  if (size == 0) w.put(2, 0);
-  else {
-    uint32_t nbits = size == 1 ? 1 : (32u - (uint32_t)__builtin_clz((uint32_t)size - 1));
-    uint32_t nbytes = (nbits + 7) / 8;
-    w.put(2, nbytes); w.put(8 * nbytes, size - 1);
-  }
-  w.align();
-  w.v.insert(w.v.end(), meta.begin(), meta.end());
-}
-int lgblock_of(const Params& p) {   /* quality.h:76 ComputeLgBlock, quality >= 2 */
-  if (p.quality < 4) return 14;
-  if (p.lgblock != 0) return p.lgblock > 24 ? 24 : p.lgblock < 16 ? 16 : p.lgblock;
-  return (p.quality >= 9 && p.lgwin > 16) ? (p.lgwin < 18 ? p.lgwin : 18) : 16;
-}
-
-// The whole stream for the operations seen so far (quality 5..9): the device compresses the accumulated input cut at the
-// positions of the FLUSH / EMIT_METADATA operations (br_kernels.cu k_assemble_scan pads behind a FLUSH); metadata blocks and
-// everything that happens before the first input byte are spliced in here.  Every call reproduces the bytes of the call
-// before as a prefix: the parse is causal, and each cut ends on a byte boundary.
-int build_wire(BrotliEncoderState* s, bool is_final, bool finish_empty, std::vector<uint8_t>& W) {
-  const size_t n = s->input.size();
-  const int lgwin = s->params.lgwin > 24 ? 24 : s->params.lgwin;
-  W.clear();
-  BitOut w{W, 0};
-  size_t e = 0;
-  const std::vector<StreamEvent>& ev = s->events;
-  const bool lead = !ev.empty() && ev[0].pos == 0;
-  const bool continued = s->params.stream_offset != 0;   /* encode.c:675: a stream that continues another one has no window bits */
-  if (lead || n == 0) {
-    if (!continued) {   // encode.c:185 EncodeWindowBits
-      if (lgwin == 16) w.put(1, 0);
-      else if (lgwin == 17) w.put(7, 1);
-      else if (lgwin > 17) w.put(4, (uint64_t)(((lgwin - 17) << 1) | 1));
-      else w.put(7, (uint64_t)(((lgwin - 8) << 4) | 1));
-    }
-    for (; e < ev.size() && ev[e].pos == 0; ++e) {
-      if (ev[e].kind == 1) { if (w.pb) { w.put(6, 6); w.align(); } }   // encode.c:1356 InjectBytePaddingBlock
-      else put_metadata(w, ev[e].meta);
-    }
-  }
-  if (n == 0) {
-    if (is_final) { w.put(2, 3); w.align(); }   // encode.c:1006: ISLAST + ISEMPTY
-    return 1;
-  }
-  std::vector<uint32_t> cut_pos, cut_kind;
-  for (size_t i = e; i < ev.size(); ++i)
-    if (cut_pos.empty() || cut_pos.back() != ev[i].pos) { cut_pos.push_back(ev[i].pos); cut_kind.push_back((uint32_t)ev[i].kind); }
-  const bool cut_at_end = !cut_pos.empty() && cut_pos.back() == n;
-  std::vector<uint64_t> end_bit(cut_pos.size() + 1, 0);
-  BrCuts c; c.pos = cut_pos.data(); c.kind = cut_kind.data(); c.n = (uint32_t)cut_pos.size();
-  c.is_final = (is_final && !cut_at_end) ? 1 : 0; c.with_header = (lead || continued) ? 0 : 1;
-  c.stream_offset = s->params.stream_offset;
-  c.finish_empty = (c.is_final && finish_empty) ? 1 : 0; c.end_bit = end_bit.data();
-  c.lgblock = s->params.lgblock; c.disable_ctx = (int)s->params.disable_ctx; c.stream_end = nullptr;
-  if (!c.is_final && !cut_at_end) return 0;   // (callers only build the wire at a cut or at FINISH)
-  std::vector<uint8_t> D;
-  size_t got = 0;
-  if (!compress_host(s->params, s->params.size_hint, s->input.data(), n, nullptr, 0, &got, &D, &c)) return 0;
-  size_t from = 0;
-  for (size_t i = 0; i < cut_pos.size(); ++i) {
-    const uint64_t eb = end_bit[i];
-    size_t upto, next;
-    if (cut_kind[i] == 1) { next = (size_t)(((eb & 7) ? eb + 6 : eb) + 7) >> 3; upto = next; }   // the device wrote the padding block
-    else { upto = (size_t)((eb + 7) >> 3); next = upto; }
-    W.insert(W.end(), D.begin() + (long)from, D.begin() + (long)upto);
-    w.pb = cut_kind[i] == 2 ? (uint32_t)(eb & 7) : 0;
-    bool first = true;
-    for (; e < ev.size() && ev[e].pos == cut_pos[i]; ++e, first = false) {
-      if (ev[e].kind == 2) put_metadata(w, ev[e].meta);   // (a FLUSH on a byte boundary emits nothing)
-      else if (!first) {}
-    }
-    w.align();
-    from = next;
-  }
-  W.insert(W.end(), D.begin() + (long)from, D.end());
-  if (is_final && cut_at_end) W.push_back(3);   // encode.c:520: empty last metablock on a byte boundary
-  return 1;
-}
-}  // namespace
 
 extern "C" {
 
@@ -446,59 +188,19 @@ int BrotliB200Available(void) {
 void BrotliB200LastStats(double out[16]) { memcpy(out, tls.last, sizeof(tls.last)); }
 void BrotliB200LastStatsQ1(double out[12]) { memcpy(out, tls.last_q1, sizeof(tls.last_q1)); }
 
-size_t BrotliEncoderMaxCompressedSize(size_t input_size) {  /* encode.c:1251 */
-  size_t num_large_blocks = input_size >> 14;
-  size_t overhead = 2 + (4 * num_large_blocks) + 3 + 1;
-  size_t result = input_size + overhead;
-  if (input_size == 0) return 2;
-  return (result < input_size) ? 0 : result;
-}
+size_t BrotliEncoderMaxCompressedSize(size_t input_size) { return max_compressed_size(input_size); }
 
 BROTLI_BOOL BrotliEncoderCompress(int quality, int lgwin, BrotliEncoderMode mode, size_t input_size,
     const uint8_t* input_buffer, size_t* encoded_size, uint8_t* encoded_buffer) {
-  size_t out_size = *encoded_size;
-  size_t max_out_size = BrotliEncoderMaxCompressedSize(input_size);
-  if (out_size == 0) return BROTLI_FALSE;
-  if (input_size == 0) { *encoded_size = 1; *encoded_buffer = 6; return BROTLI_TRUE; }
-  Params p; p.quality = quality; p.lgwin = lgwin; p.mode = mode;
-  p.size_hint = (uint32_t)input_size;
-  if (lgwin > 24) p.large_window = 1;
-  if (!supported(p)) { *encoded_size = 0; return BROTLI_FALSE; }
-  size_t got = 0;
-  int ok;
-  if (quality == 1) {
-    std::vector<uint8_t> tmp; Q1Tail tail;
-    ok = q1_run(p, input_buffer, input_size, nullptr, 0, 2, tail, tmp);
-    got = tmp.size();
-    if (ok && got <= max_out_size) {
-      if (got > out_size) ok = 2;
-      else memcpy(encoded_buffer, tmp.data(), got);
-    }
-  } else {
-    ok = compress_host(p, (uint32_t)input_size, input_buffer, input_size, encoded_buffer, out_size, &got, nullptr);
-  }
-  if (ok == 1 && !(max_out_size && got > max_out_size)) { *encoded_size = got; return BROTLI_TRUE; }
-  *encoded_size = 0;
-  if (!ok) return BROTLI_FALSE;   /* GPU path failed: fail loudly, never substitute other bytes */
-  /* ok == 2: the stream did not fit the caller's buffer -- the reference's "not finished" case, same fallback */
-  /* encode.c:1345: result larger than BrotliEncoderMaxCompressedSize -> raw stream */
-  if (!max_out_size) return BROTLI_FALSE;
-  if (out_size >= max_out_size) {
-    *encoded_size = make_uncompressed_stream(input_buffer, input_size, encoded_buffer);
-    return BROTLI_TRUE;
-  }
-  return BROTLI_FALSE;
+  return compress_oneshot(kDevice, quality, lgwin, mode, input_size, input_buffer, encoded_size, encoded_buffer);
 }
 
 BROTLI_BOOL BrotliB200CompressDevice(int quality, int lgwin, size_t input_size, const void* d_input,
                                      size_t* encoded_size, void* d_encoded) {
-  Params p; p.quality = quality; p.lgwin = lgwin;
-  if (lgwin > 24) p.large_window = 1;   /* as the one-shot wrapper (encode.c:1329): refused unless quality <= 2 drops it again */
+  const Params p = oneshot_params(quality, lgwin);
   if (!supported(p) || input_size == 0 || input_size > (1u << 30) || !ensure_job()) return BROTLI_FALSE;
   const uint8_t* d_out = nullptr; size_t sz = 0;
-  if (lgwin < 10) lgwin = 10;   /* quality.h:60 SanitizeParams */
-  if (lgwin > 24) lgwin = 24;   /* (only quality <= 2 gets here with more: no large window there, quality.h:63) */
-  if (!br_job_compress_device(tls.job, quality, lgwin, (uint32_t)input_size, (const uint8_t*)d_input,
+  if (!br_job_compress_device(tls.job, quality, window_of(p), (uint32_t)input_size, (const uint8_t*)d_input,
                               (uint32_t)input_size, &d_out, &sz, nullptr)) return BROTLI_FALSE;
   record_stats();
   if (sz > *encoded_size) return BROTLI_FALSE;
@@ -512,48 +214,36 @@ BROTLI_BOOL BrotliB200CompressDevice(int quality, int lgwin, size_t input_size, 
 size_t BrotliB200CompressBatch(int quality, int lgwin, size_t count, const uint8_t* const* inputs,
     const size_t* input_sizes, uint8_t* const* outputs, size_t* encoded_sizes, int threads) {
   if (threads < 1) threads = 1;
+  const Params p = oneshot_params(quality, lgwin);
+  if (!supported(p) || (quality == 1 && count && !ensure_q1())) { for (size_t i = 0; i < count; ++i) encoded_sizes[i] = 0; return 0; }
   if (quality == 1 && count) {
     /* one device batch: all streams through the same four launches (br_q1.cu) */
-    Params p; p.quality = 1; p.lgwin = lgwin;
-    if (!supported(p) || !ensure_q1()) { for (size_t i = 0; i < count; ++i) encoded_sizes[i] = 0; return 0; }
-    int w = lgwin < 10 ? 10 : lgwin > 24 ? 24 : lgwin;   /* quality.h:60-69 (no large window at quality <= 2) */
     std::vector<int> ok(count, 0);
     std::vector<size_t> caps(encoded_sizes, encoded_sizes + count);
-    br_q1_compress_batch(tls.q1, w, count, inputs, input_sizes, nullptr, nullptr, nullptr, outputs, encoded_sizes, ok.data(), threads, 1, 2, nullptr, nullptr);
+    br_q1_compress_batch(tls.q1, window_of(p), count, inputs, input_sizes, nullptr, nullptr, nullptr, outputs, encoded_sizes, ok.data(), threads, 1, 2, nullptr, nullptr);
     record_q1_stats();
     size_t good = 0;
     for (size_t i = 0; i < count; ++i) {
       /* what the one-shot wrapper adds per stream: encode.c:1310 (empty input) and :1345 (raw-stream rule) */
-      const size_t bound = BrotliEncoderMaxCompressedSize(input_sizes[i]);
       if (input_sizes[i] == 0) {
         if (caps[i] >= 1) { outputs[i][0] = 6; encoded_sizes[i] = 1; ++good; } else encoded_sizes[i] = 0;
-      } else if (ok[i] && encoded_sizes[i] <= bound) {
-        ++good;
-      } else if (ok[i] && caps[i] >= bound) {
-        encoded_sizes[i] = make_uncompressed_stream(inputs[i], input_sizes[i], outputs[i]); ++good;
-      } else {
-        encoded_sizes[i] = 0;
+        continue;
+      }
+      switch (ok[i] ? fit_stream(encoded_sizes[i], caps[i], input_sizes[i]) : kFail) {
+        case kKeep: ++good; break;
+        case kRaw: encoded_sizes[i] = make_uncompressed_stream(inputs[i], input_sizes[i], outputs[i]); ++good; break;
+        default: encoded_sizes[i] = 0;
       }
     }
     return good;
   }
-  /* quality 2..9: streams below 1 MiB go through the device in groups (one job per group, compress_stream_group); longer
-     ones one by one, `threads` host workers each with its own CUDA stream */
-  Params p; p.quality = quality; p.lgwin = lgwin;
-  if (lgwin > 24) p.large_window = 1;
-  if (!supported(p)) { for (size_t i = 0; i < count; ++i) encoded_sizes[i] = 0; return 0; }
+  /* quality 2..9: streams below 1 MiB go through the device in groups (compress_stream_group); the others one by one,
+     `threads` host workers each with its own CUDA stream */
+  std::vector<std::vector<size_t>> groups;
+  std::vector<size_t> big;
+  plan_groups(input_sizes, count, groups, big);
   size_t ok = 0;
-  std::vector<size_t> big, group;
-  size_t group_bytes = 0;
-  for (size_t i = 0; i < count; ++i) {
-    if (input_sizes[i] == 0 || input_sizes[i] >= ((size_t)1 << 20)) { big.push_back(i); continue; }
-    if ((group_bytes + input_sizes[i] > kBatchGroupBytes || group.size() >= kBatchGroupStreams) && !group.empty()) {
-      ok += compress_stream_group(quality, lgwin, group, inputs, input_sizes, outputs, encoded_sizes, threads);
-      group.clear(); group_bytes = 0;
-    }
-    group.push_back(i); group_bytes += input_sizes[i];
-  }
-  if (!group.empty()) ok += compress_stream_group(quality, lgwin, group, inputs, input_sizes, outputs, encoded_sizes, threads);
+  for (const std::vector<size_t>& g : groups) ok += compress_stream_group(p, g, inputs, input_sizes, outputs, encoded_sizes, threads);
   if (big.empty()) return ok;
   if ((size_t)threads > big.size()) threads = (int)big.size();
   std::vector<size_t> okc((size_t)threads, 0);
@@ -576,67 +266,52 @@ size_t BrotliB200CompressBatch(int quality, int lgwin, size_t count, const uint8
 
 size_t BrotliB200CompressBatchDevice(int quality, int lgwin, size_t count, const void* d_inputs, const uint64_t* input_offsets,
     const size_t* input_sizes, void* d_encoded, size_t encoded_capacity, uint64_t* encoded_offsets, size_t* encoded_sizes) {
-  Params p; p.quality = quality; p.lgwin = lgwin;
-  if (lgwin > 24) p.large_window = 1;
+  const Params p = oneshot_params(quality, lgwin);
   if (!count || !supported(p)) return 0;
   for (size_t i = 0; i < count; ++i) if (input_sizes[i] == 0) return 0;
+  /* encode.c:1345: above BrotliEncoderMaxCompressedSize the one-shot wrapper substitutes the raw stream, which needs the
+     host copy of the input: such a stream is reported as failed here (size 0) */
   if (quality != 1) {
-    /* quality 2..9: streams below 1 MiB, consecutive ones grouped into device jobs of <= 128 MiB / 8192 streams (the job
-       of compress_stream_group, without the host staging): a group whose streams lie back to back in d_inputs is read
-       in place, otherwise it is gathered with device copies; the job's output is dense and goes to d_encoded as it is. */
-    for (size_t i = 0; i < count; ++i) if (input_sizes[i] >= ((size_t)1 << 20)) return 0;   /* longer streams: BrotliB200CompressDevice */
-    if (!ensure_job()) return 0;
+    /* quality 2..9: streams below 1 MiB (longer ones: BrotliB200CompressDevice) in the groups of compress_stream_group,
+       without the host staging: a group whose streams lie back to back in d_inputs is read in place, otherwise it is
+       gathered with device copies; the job's output is dense and goes to d_encoded as it is. */
+    std::vector<std::vector<size_t>> groups;
+    std::vector<size_t> single;
+    plan_groups(input_sizes, count, groups, single);
+    if (!single.empty() || !ensure_job()) return 0;
     cudaStream_t st = (cudaStream_t)br_job_stream(tls.job);
-    const int w = lgwin > 24 ? 24 : lgwin < 10 ? 10 : lgwin;
     const uint8_t* din = (const uint8_t*)d_inputs;
     uint8_t* dout = (uint8_t*)d_encoded;
-    size_t used = 0, good = 0, a = 0;
+    size_t used = 0, good = 0, a = 0;   // a: the first stream of the group (groups are consecutive, in order)
     for (size_t i = 0; i < count; ++i) encoded_sizes[i] = 0;
     bool failed = false;
-    while (a < count && !failed) {
-      size_t b = a, n = 0; uint32_t hint = 0; bool packed = true;
-      while (b < count && b - a < kBatchGroupStreams && n + input_sizes[b] <= kBatchGroupBytes) {
-        if (b > a && input_offsets[b] != input_offsets[b - 1] + input_sizes[b - 1]) packed = false;
-        if (input_sizes[b] > hint) hint = (uint32_t)input_sizes[b];
-        n += input_sizes[b]; ++b;
-      }
-      const size_t k = b - a;
+    for (const std::vector<size_t>& idx : groups) {
+      const size_t k = idx.size();
+      GroupCuts g(input_sizes + a, nullptr, k);
+      bool packed = true;
+      for (size_t j = a + 1; j < a + k; ++j) if (input_offsets[j] != input_offsets[j - 1] + input_sizes[j - 1]) packed = false;
       const uint8_t* src = din + input_offsets[a];
       if (!packed) {
-        if (tls.d_in_cap < n) {
-          if (tls.d_in) cudaFree(tls.d_in);
-          tls.d_in = nullptr; tls.d_in_cap = 0;
-          if (cudaMalloc(&tls.d_in, n + 64) != cudaSuccess) { cudaGetLastError(); failed = true; break; }
-          tls.d_in_cap = n;
-        }
-        size_t o = 0;
-        for (size_t j = a; j < b && !failed; ++j) {
-          if (cudaMemcpyAsync(tls.d_in + o, din + input_offsets[j], input_sizes[j], cudaMemcpyDeviceToDevice, st) != cudaSuccess) failed = true;
-          o += input_sizes[j];
-        }
+        if (!reserve_d_in(g.n)) { failed = true; break; }
+        for (size_t j = 0; j < k && !failed; ++j)
+          if (cudaMemcpyAsync(tls.d_in + (j ? g.pos[j - 1] : 0), din + input_offsets[a + j], input_sizes[a + j], cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+            failed = true;
         if (failed) break;
         src = tls.d_in;
       }
-      std::vector<uint32_t> pos(k, 0), kind(k, 3);
-      { size_t o = 0; for (size_t j = 0; j + 1 < k; ++j) { o += input_sizes[a + j]; pos[j] = (uint32_t)o; } }
-      std::vector<uint64_t> ends(k + 1, 0);
-      BrCuts c; memset(&c, 0, sizeof(c));
-      c.pos = pos.data(); c.kind = kind.data(); c.n = (uint32_t)(k - 1); c.is_final = 1; c.with_header = 1; c.stream_end = ends.data();
       const uint8_t* d_o = nullptr; size_t sz = 0;
-      if (!br_job_compress_device(tls.job, quality, w, hint, src, (uint32_t)n, &d_o, &sz, k > 1 ? &c : nullptr)) { failed = true; break; }
+      if (!br_job_compress_device(tls.job, quality, window_of(p), g.hint, src, (uint32_t)g.n, &d_o, &sz, k > 1 ? &g.c : nullptr)) { failed = true; break; }
       record_stats();
-      if (k == 1) ends[0] = sz;
-      if (ends[k - 1] != sz || used + sz > encoded_capacity) { failed = true; break; }
+      if (k == 1) g.ends[0] = sz;
+      if (g.ends[k - 1] != sz || used + sz > encoded_capacity) { failed = true; break; }
       if (cudaMemcpyAsync(dout + used, d_o, sz, cudaMemcpyDeviceToDevice, st) != cudaSuccess) { failed = true; break; }
       for (size_t j = 0; j < k; ++j) {
-        const size_t from = j ? (size_t)ends[j - 1] : 0, got = (size_t)ends[j] - from;
+        const size_t from = j ? (size_t)g.ends[j - 1] : 0, got = (size_t)g.ends[j] - from;
         encoded_offsets[a + j] = used + from;
-        /* encode.c:1345: above BrotliEncoderMaxCompressedSize the one-shot wrapper substitutes the raw stream, which needs
-           the host copy of the input: such a stream is reported as failed here (size 0), like at quality 1 */
-        if (got <= BrotliEncoderMaxCompressedSize(input_sizes[a + j])) { encoded_sizes[a + j] = got; ++good; }
+        if (within_bound(got, input_sizes[a + j])) { encoded_sizes[a + j] = got; ++good; }
       }
       used += sz;
-      a = b;
+      a += k;
     }
     for (size_t i = a; i < count; ++i) encoded_offsets[i] = used;   /* (streams behind a failure) */
     encoded_offsets[count] = used;
@@ -647,14 +322,11 @@ size_t BrotliB200CompressBatchDevice(int quality, int lgwin, size_t count, const
   BrQ1Packed pk; pk.d_in = (const uint8_t*)d_inputs; pk.in_off = input_offsets; pk.d_out = (uint8_t*)d_encoded;
   pk.out_cap = encoded_capacity; pk.out_off = encoded_offsets;
   std::vector<int> ok(count, 0);
-  int w = lgwin < 10 ? 10 : lgwin > 24 ? 24 : lgwin;
-  if (!br_q1_compress_batch(tls.q1, w, count, nullptr, input_sizes, nullptr, nullptr, &pk, nullptr, encoded_sizes, ok.data(), 1, 1, 2, nullptr, nullptr)) return 0;
+  if (!br_q1_compress_batch(tls.q1, window_of(p), count, nullptr, input_sizes, nullptr, nullptr, &pk, nullptr, encoded_sizes, ok.data(), 1, 1, 2, nullptr, nullptr)) return 0;
   record_q1_stats();
   size_t good = 0;
   for (size_t i = 0; i < count; ++i) {
-    /* encode.c:1345: a stream above BrotliEncoderMaxCompressedSize is replaced by the raw stream in the one-shot
-       wrapper; that rewrite needs the host copy of the input, so such a stream is reported as failed here */
-    if (encoded_sizes[i] <= BrotliEncoderMaxCompressedSize(input_sizes[i])) ++good; else encoded_sizes[i] = 0;
+    if (within_bound(encoded_sizes[i], input_sizes[i])) ++good; else encoded_sizes[i] = 0;
   }
   return good;
 }
@@ -673,27 +345,8 @@ void BrotliEncoderDestroyInstance(BrotliEncoderState* state) {
 }
 
 BROTLI_BOOL BrotliEncoderSetParameter(BrotliEncoderState* s, BrotliEncoderParameter p, uint32_t value) {
-  if (s->initialized) return BROTLI_FALSE;   /* encode.c:63 */
-  switch (p) {
-    case BROTLI_PARAM_MODE: s->params.mode = (int)value; return BROTLI_TRUE;
-    case BROTLI_PARAM_QUALITY: s->params.quality = (int)value; return BROTLI_TRUE;
-    case BROTLI_PARAM_LGWIN: s->params.lgwin = (int)value; return BROTLI_TRUE;
-    case BROTLI_PARAM_LGBLOCK: s->params.lgblock = (int)value; return BROTLI_TRUE;
-    case BROTLI_PARAM_DISABLE_LITERAL_CONTEXT_MODELING:
-      if (value != 0 && value != 1) return BROTLI_FALSE;
-      s->params.disable_ctx = value; return BROTLI_TRUE;
-    case BROTLI_PARAM_SIZE_HINT: s->params.size_hint = value; return BROTLI_TRUE;
-    case BROTLI_PARAM_LARGE_WINDOW: s->params.large_window = !!value; return BROTLI_TRUE;
-    case BROTLI_PARAM_NPOSTFIX: s->params.npostfix = value; return BROTLI_TRUE;
-    case BROTLI_PARAM_NDIRECT: s->params.ndirect = value; return BROTLI_TRUE;
-    case BROTLI_PARAM_STREAM_OFFSET:
-      if (value > (1u << 30)) return BROTLI_FALSE;
-      s->params.stream_offset = value; return BROTLI_TRUE;
-    case BROTLI_PARAM_BASE64_MODE: s->params.base64 = value & 1; return BROTLI_TRUE;
-    case BROTLI_PARAM_MAX_BASE64_REGIONS: return BROTLI_TRUE;
-    case BROTLI_PARAM_SIMD_HASHER: return value > 2 ? BROTLI_FALSE : BROTLI_TRUE;  /* output-equivalent */
-    default: return BROTLI_FALSE;
-  }
+  if (s->s.initialized) return BROTLI_FALSE;   /* encode.c:63 */
+  return set_parameter(s->s.params, p, value);
 }
 
 BrotliEncoderPreparedDictionary* BrotliEncoderPrepareDictionary(BrotliSharedDictionaryType, size_t, const uint8_t*, int,
@@ -703,133 +356,14 @@ BROTLI_BOOL BrotliEncoderAttachPreparedDictionary(BrotliEncoderState*, const Bro
   return BROTLI_FALSE;
 }
 
-static void push_output(BrotliEncoderState* s, size_t* available_out, uint8_t** next_out, size_t* total_out) {
-  size_t avail = s->output.size() - s->out_pos;
-  if (avail && *available_out && next_out && *next_out) {
-    size_t c = avail < *available_out ? avail : *available_out;
-    memcpy(*next_out, s->output.data() + s->out_pos, c);
-    *next_out += c; *available_out -= c; s->out_pos += c; s->total_out += c;
-  }
-  if (total_out) *total_out = (size_t)s->total_out;
-}
-
-/* encode.c:1634.  Quality 5..9: the input is accumulated on the host; every FLUSH / EMIT_METADATA / FINISH sends the
-   whole stream so far through the GPU pipeline, cut where those operations happened (build_wire), and hands out the bytes
-   that are new.  The bytes equal the reference's for the same call sequence (SURVEY.md section 0, T6: the size hint is frozen
-   when the reference would have frozen it, at its first EncodeData call).  Cost: a stream with k flushes is compressed k
-   times, and host memory grows with the stream (at most 1 GiB, then PROCESS fails) -- the reference's bounded-memory
-   streaming needs the pipeline to resume from a saved window, which it does not do yet.
-   Quality 1 (encode.c:1425): every call compresses its own fragments; FLUSH is cheap. */
-static BROTLI_BOOL compress_stream_impl(BrotliEncoderState* s, BrotliEncoderOperation op, size_t* available_in,
-    const uint8_t** next_in, size_t* available_out, uint8_t** next_out, size_t* total_out);
 BROTLI_BOOL BrotliEncoderCompressStream(BrotliEncoderState* s, BrotliEncoderOperation op, size_t* available_in,
     const uint8_t** next_in, size_t* available_out, uint8_t** next_out, size_t* total_out) {
-  try { return compress_stream_impl(s, op, available_in, next_in, available_out, next_out, total_out); }
+  try { return compress_stream(kDevice, s->s, op, available_in, next_in, available_out, next_out, total_out); }
   catch (const std::bad_alloc&) { return BROTLI_FALSE; }   /* the reference reports allocation failure the same way */
 }
-static BROTLI_BOOL compress_stream_impl(BrotliEncoderState* s, BrotliEncoderOperation op, size_t* available_in,
-    const uint8_t** next_in, size_t* available_out, uint8_t** next_out, size_t* total_out) {
-  s->initialized = true;
-  const bool q1 = s->params.quality == 1;
-  if (!supported(s->params)) return BROTLI_FALSE;
-  if (op == BROTLI_OPERATION_EMIT_METADATA && q1) return BROTLI_FALSE;   /* not built for the fragment coder */
-  if (s->compressed && (*available_in != 0 || op == BROTLI_OPERATION_EMIT_METADATA)) return BROTLI_FALSE;   /* input after finish */
-  if (!q1 && !s->compressed) {
-    /* ---- quality 5..9 */
-    if (op == BROTLI_OPERATION_EMIT_METADATA) {
-      if (*available_in > (1u << 24)) return BROTLI_FALSE;   /* encode.c:1552 */
-    } else if (*available_in) {
-      if (s->input.size() + *available_in > ((size_t)1 << 30)) return BROTLI_FALSE;   /* positions are 32-bit in the pipeline */
-      s->input.insert(s->input.end(), *next_in, *next_in + *available_in);
-    }
-    const bool finish_without_input = op == BROTLI_OPERATION_FINISH && *available_in == 0;
-    if (!s->hint_fixed) {
-      /* encode.c:1619 UpdateSizeHint runs at the first EncodeData: when the first input block (1 << lgblock) is full
-         or the operation is not PROCESS. */
-      if (op != BROTLI_OPERATION_PROCESS || s->input.size() >= ((size_t)1 << lgblock_of(s->params)) ||
-          (s->params.stream_offset && s->input.size() >= 2)) {
-        /* (an estimate of zero -- an operation before any input -- is taken again at the next EncodeData) */
-        if (s->params.size_hint == 0) s->params.size_hint = (uint32_t)s->input.size();
-        s->hint_fixed = s->params.size_hint != 0;
-      }
-    }
-    if (s->params.stream_offset && !s->flint_done && s->input.size() >= 2 &&
-        !(s->input.size() == 2 && op == BROTLI_OPERATION_FINISH)) {
-      /* encode.c:1704: with a stream offset the first two bytes are flushed on their own (unless the stream ends there) */
-      StreamEvent e; e.pos = 2; e.kind = 1;
-      s->events.push_back(std::move(e));
-      s->flint_done = true;
-    }
-    if (op == BROTLI_OPERATION_EMIT_METADATA) {
-      StreamEvent e; e.pos = (uint32_t)s->input.size(); e.kind = 2; e.meta.assign(*next_in, *next_in + *available_in);
-      s->events.push_back(std::move(e));
-    } else if (op == BROTLI_OPERATION_FLUSH) {
-      StreamEvent e; e.pos = (uint32_t)s->input.size(); e.kind = 1;
-      s->events.push_back(std::move(e));
-    }
-    if (op != BROTLI_OPERATION_EMIT_METADATA) *next_in += *available_in;
-    else *next_in += *available_in;
-    *available_in = 0;
-    if (op != BROTLI_OPERATION_PROCESS) {
-      const size_t last_cut = s->events.empty() ? 0 : s->events.back().pos;
-      const size_t bs = (size_t)1 << lgblock_of(s->params);
-      /* FINISH without input right behind a full input block: that block was already encoded as a non-last one */
-      const bool finish_empty = finish_without_input && s->input.size() > last_cut && (s->input.size() - last_cut) % bs == 0;
-      std::vector<uint8_t> W;
-      if (!build_wire(s, op == BROTLI_OPERATION_FINISH, finish_empty, W)) return BROTLI_FALSE;
-      if (W.size() < s->wire_sent) return BROTLI_FALSE;
-      s->output.erase(s->output.begin(), s->output.begin() + (long)s->out_pos); s->out_pos = 0;
-      s->output.insert(s->output.end(), W.begin() + (long)s->wire_sent, W.end());
-      s->wire_sent = W.size();
-      if (op == BROTLI_OPERATION_FINISH) { s->compressed = true; ByteVec(s->input.get_allocator()).swap(s->input); }
-    }
-    push_output(s, available_out, next_out, total_out);
-    if (s->compressed && s->out_pos == s->output.size()) s->finished = true;
-    return BROTLI_TRUE;
-  }
-  /* ---- quality 1 (encode.c:1425): the reference compresses the fragments of every call at once.  Here calls are
-     collected (their sizes recorded: they decide the fragments) and run through the device as one segment when the
-     operation is FLUSH / FINISH or kQ1SegmentBytes / 2 of input are waiting, so memory stays bounded and a stream has no
-     size limit; between segments only the pending bits of the last byte are kept (Q1Tail). */
-  if (!s->compressed) {
-    if (*available_in || op == BROTLI_OPERATION_FINISH) s->calls.push_back(*available_in);
-    if (*available_in) {
-      s->input.insert(s->input.end(), *next_in, *next_in + *available_in);
-      *next_in += *available_in; *available_in = 0;
-    }
-    if (op != BROTLI_OPERATION_PROCESS || s->input.size() >= kQ1SegmentBytes / 2) {
-      const int end_op = op == BROTLI_OPERATION_FINISH ? 2 : op == BROTLI_OPERATION_FLUSH ? 1 : 0;
-      s->output.erase(s->output.begin(), s->output.begin() + (long)s->out_pos); s->out_pos = 0;
-      if (!q1_run(s->params, s->input.data(), s->input.size(), s->calls.data(), s->calls.size(), end_op, s->q1_tail, s->output))
-        return BROTLI_FALSE;
-      s->input.clear(); s->calls.clear();
-      if (op == BROTLI_OPERATION_FINISH) { s->compressed = true; ByteVec(s->input.get_allocator()).swap(s->input); }
-    }
-  }
-  push_output(s, available_out, next_out, total_out);
-  if (s->compressed && s->out_pos == s->output.size()) s->finished = true;
-  return BROTLI_TRUE;
-}
 
-BROTLI_BOOL BrotliEncoderIsFinished(BrotliEncoderState* s) {
-  return (s->compressed && s->out_pos == s->output.size()) ? BROTLI_TRUE : BROTLI_FALSE;
-}
-BROTLI_BOOL BrotliEncoderHasMoreOutput(BrotliEncoderState* s) {
-  return s->out_pos < s->output.size() ? BROTLI_TRUE : BROTLI_FALSE;
-}
-const uint8_t* BrotliEncoderTakeOutput(BrotliEncoderState* s, size_t* size) {   /* encode.c:1742 */
-  size_t avail = s->output.size() - s->out_pos;
-  size_t consumed = avail;
-  const uint8_t* result = nullptr;
-  if (*size) consumed = *size < avail ? *size : avail;
-  if (consumed) {
-    result = s->output.data() + s->out_pos;
-    s->out_pos += consumed; s->total_out += consumed;
-    *size = consumed;
-  } else {
-    *size = 0;
-  }
-  return result;
-}
+BROTLI_BOOL BrotliEncoderIsFinished(BrotliEncoderState* s) { return is_finished(s->s) ? BROTLI_TRUE : BROTLI_FALSE; }
+BROTLI_BOOL BrotliEncoderHasMoreOutput(BrotliEncoderState* s) { return has_more_output(s->s) ? BROTLI_TRUE : BROTLI_FALSE; }
+const uint8_t* BrotliEncoderTakeOutput(BrotliEncoderState* s, size_t* size) { return take_output(s->s, size); }
 
 }  // extern "C"

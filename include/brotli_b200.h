@@ -28,7 +28,7 @@
  *   are the newest path: see DESIGN.md section 3d for what has and has not been run on a GPU.)  BROTLI_PARAM_LGBLOCK, DISABLE_LITERAL_CONTEXT_MODELING, SIZE_HINT and (quality 5..9)
  *   STREAM_OFFSET are honoured.  Quality 1: streams of any size, compressed in device segments of <= 128 MiB as the calls
  *   arrive (bounded memory).  Quality 2..9: one stream <= 1 GiB -- BrotliEncoderCompressStream fails on the PROCESS call
- *   that crosses it; the stream so far is kept in host memory and recompressed at every FLUSH (see csrc/br_api.cc).
+ *   that crosses it; the stream so far is kept in host memory and recompressed at every FLUSH (see csrc/br_driver.h).
  *   FLUSH, FINISH and (quality 2..9) EMIT_METADATA follow encode.h:93-157. */
 #include <brotli/encode.h>
 #ifdef __cplusplus

@@ -650,15 +650,17 @@ extern "C" long sim_q1_compress(int lgwin, const u8* in, u32 n, const size_t* ca
 #endif
 
 #ifdef BR_SIM_ENTROPY
+#include "../../brotli_b200/csrc/br_driver.h"
 // A batch of independent streams laid end to end (cuts of kind 3, br_pipeline.h): bounds[k] = end of stream k (bounds[ns-1] = n).
 // stream_end[k] receives the byte offset where stream k ends in `out`.
 static long sim_compress_multi_impl(int q, int lgwin, const u8* in, u32 n, const u32* bounds, u32 nstreams, u64* stream_end,
                                     u8* out, size_t out_cap, u32* stats, const SimSched* sched, u32 nstats) {
-  std::vector<u32> kind(nstreams, 3);
-  u32 hint = 0;
-  for (u32 k = 0; k < nstreams; ++k) { const u32 sz = bounds[k] - (k ? bounds[k - 1] : 0); if (sz > hint) hint = sz; }
-  const BrCuts c = {bounds, kind.data(), nstreams - 1, 1, 1, 0, nullptr, 0, 0, 0, stream_end};
-  return sim_compress_impl(q, lgwin, hint, in, n, out, out_cap, stats, &c, sched, nstats);
+  std::vector<size_t> sizes(nstreams);
+  for (u32 k = 0; k < nstreams; ++k) sizes[k] = bounds[k] - (k ? bounds[k - 1] : 0);
+  br_driver::GroupCuts g(sizes.data(), nullptr, nstreams);
+  const long r = sim_compress_impl(q, lgwin, g.hint, in, n, out, out_cap, stats, &g.c, sched, nstats);
+  if (r >= 0 && stream_end) std::copy(g.ends.begin(), g.ends.begin() + nstreams, stream_end);
+  return r;
 }
 extern "C" long sim_compress_multi(int q, int lgwin, const u8* in, u32 n, const u32* bounds, u32 nstreams, u64* stream_end,
                                    u8* out, size_t out_cap, u32* stats) {
@@ -679,5 +681,86 @@ extern "C" long sim_compress_sched(int q, int lgwin, const u8* in, u32 n, const 
   }
   const BrCuts c = {cut_pos, cut_kind, ncuts, 1, 1, 0, nullptr, 0, 0, 0, nullptr};
   return sim_compress_impl(q, lgwin, size_hint, in, n, out, out_cap, stats, ncuts ? &c : nullptr, sched, SIM_ST_WORDS);
+}
+
+// ------------------------------------------------------------------ the C API's host driver (br_driver.h) over the sim
+// The driver's backend: sim_compress_impl and sim_q1_compress_seg stand in for the device pipelines.
+static int sim_backend_compress(const br_driver::Params& p, u32 size_hint, const u8* in, size_t n, const BrCuts* cuts, u8* out,
+                                size_t cap, size_t* got, std::vector<u8>* vec) {
+  if (!br_driver::supported(p) || n == 0 || n > (1u << 30)) return 0;
+  std::vector<u8> res(n + n / 2 + 4096 + 64 * (size_t)(cuts ? cuts->n : 0));
+  u32 st[SIM_ST_WORDS];
+  const long r = sim_compress_impl(p.quality, br_driver::window_of(p), size_hint, in, (u32)n, res.data(), res.size(), st, cuts);
+  if (r < 0) return 0;
+  res.resize((size_t)r);
+  *got = res.size();
+  if (vec) { vec->swap(res); return 1; }
+  if (res.size() > cap) return 2;
+  memcpy(out, res.data(), res.size());
+  return 1;
+}
+static int sim_backend_q1_segment(int lgwin, const u8* in, size_t n, const std::vector<size_t>& calls, int with_header, int end_op,
+                                  u32 start_bits, u32* end_bit, std::vector<u8>& out) {
+  out.resize(2 * n + 100000);
+  const long r = sim_q1_compress_seg(lgwin, in, (u32)n, calls.data(), calls.size(), out.data(), out.size(), with_header, end_op,
+                                     start_bits, end_bit);
+  if (r < 0) return 0;
+  out.resize((size_t)r);
+  return 1;
+}
+static const br_driver::Backend kSimBackend = {sim_backend_compress, sim_backend_q1_segment};
+
+// A sequence of BrotliEncoderCompressStream calls through the driver, as tests/brotli_libs.py ref_stream_ops sends them to
+// the reference: quality, lgwin and nparams further (BrotliEncoderParameter id, value) pairs; call i hands sizes[i] bytes
+// of `data` (from where the call before stopped) with operation ops[i], and the output is drained in 64 KiB pieces until
+// the input is taken and no output is left.  q1_segment_bytes (0: the product's) is the input of one quality-1 segment.
+// Returns the stream's size in `out`, -1 when a call fails, -2 when `cap` is too small.
+extern "C" long sim_stream_ops(int q, int lgwin, const u32* param_ids, const u32* param_vals, u32 nparams, const u8* data,
+                               const size_t* sizes, const int* ops, size_t n_ops, size_t q1_segment_bytes, u8* out, size_t cap) {
+  br_driver::Stream s{br_driver::BrAlloc<u8>()};
+  br_driver::set_parameter(s.params, BROTLI_PARAM_QUALITY, (u32)q);
+  br_driver::set_parameter(s.params, BROTLI_PARAM_LGWIN, (u32)lgwin);
+  for (u32 i = 0; i < nparams; ++i)
+    if (!br_driver::set_parameter(s.params, (BrotliEncoderParameter)param_ids[i], param_vals[i])) return -1;
+  if (q1_segment_bytes) s.q1_segment_bytes = q1_segment_bytes;
+  std::vector<u8> buf(1 << 16);
+  size_t got = 0, pos = 0;
+  try {
+    for (size_t i = 0; i < n_ops; ++i) {
+      size_t avail_in = sizes[i];
+      const u8* next_in = data + pos;
+      pos += sizes[i];
+      for (;;) {
+        size_t avail_out = buf.size();
+        u8* next_out = buf.data();
+        if (!br_driver::compress_stream(kSimBackend, s, (BrotliEncoderOperation)ops[i], &avail_in, &next_in, &avail_out, &next_out,
+                                        nullptr))
+          return -1;
+        const size_t k = buf.size() - avail_out;
+        if (got + k > cap) return -2;
+        memcpy(out + got, buf.data(), k);
+        got += k;
+        if (avail_in == 0 && !br_driver::has_more_output(s)) break;
+      }
+    }
+  } catch (const std::bad_alloc&) { return -1; }
+  return (long)got;
+}
+
+// br_driver::plan_groups: group_of[i] receives the group of stream i, or -1 for a stream that goes one by one.  Returns the
+// number of groups.
+extern "C" size_t sim_plan_groups(const size_t* sizes, size_t count, long* group_of) {
+  std::vector<std::vector<size_t>> groups;
+  std::vector<size_t> single;
+  br_driver::plan_groups(sizes, count, groups, single);
+  for (size_t i : single) group_of[i] = -1;
+  for (size_t g = 0; g < groups.size(); ++g)
+    for (size_t i : groups[g]) group_of[i] = (long)g;
+  return groups.size();
+}
+
+// BrotliEncoderCompress through the driver: *encoded_size is the capacity of `out` in, the size out.  Returns the BROTLI_BOOL.
+extern "C" int sim_compress_oneshot(int q, int lgwin, const u8* in, size_t n, size_t* encoded_size, u8* out) {
+  return br_driver::compress_oneshot(kSimBackend, q, lgwin, BROTLI_MODE_GENERIC, n, in, encoded_size, out);
 }
 #endif

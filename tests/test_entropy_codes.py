@@ -101,7 +101,7 @@ def test_gpu_raw_metablocks_between_compressed(b200, oracle):
 @pytest.mark.gpu
 @pytest.mark.parametrize("q", [4, 5])
 def test_gpu_batch_of_tiny_streams(b200, oracle, q):
-    """8 192 tiny streams, one device job (br_api.cc kBatchGroupStreams): over 24 000 codes for the thread workers."""
+    """8 192 tiny streams, one device job (br_driver.h kBatchGroupStreams): over 24 000 codes for the thread workers."""
     items = _tiny_streams(8192, 920 + q)
     got = b200.compress_batch(items, q, 22, threads=4)
     for k, x in enumerate(items):
@@ -561,7 +561,7 @@ def _many_code_streams(count, seed):
 
 @pytest.mark.gpu
 def test_gpu_batch_more_codes_than_thread_workers(b200, oracle):
-    """8 192 streams of a few KiB in one device job (br_api.cc: at most 8 192 streams, under 128 MiB, each under 1 MiB)
+    """8 192 streams of a few KiB in one device job (br_driver.h: at most 8 192 streams, under 128 MiB, each under 1 MiB)
     with at least 1.5 * 65 536 prefix codes in all: more codes than the job's 65 536 thread workers, so workers build and
     store a second code over their tree area.  Each stream's bytes equal the oracle's."""
     items = _many_code_streams(8192, 930)

@@ -22,7 +22,7 @@ from brotli_libs import ROOT, TABLES, Oracle, RecordedRef
 CASES = entropy_cases.cases()
 IDS = [c[0] for c in CASES]
 SIM_SO = os.path.join(ROOT, "tests", "sim", "libbrsim.so")
-BATCH_LIMIT = 1 << 20            # streams below 1 MiB take the batch path (br_api.cc)
+BATCH_LIMIT = 1 << 20            # streams below 1 MiB take the batch path (br_driver.h)
 
 
 @pytest.fixture(scope="module")

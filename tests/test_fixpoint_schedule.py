@@ -50,7 +50,7 @@ def sched(**kw):
 def sim(tmp_path_factory):
     so = str(tmp_path_factory.mktemp("sched") / "libbrsim_sched.so")
     subprocess.check_call(["g++", "-O2", "-DBR_SIM_ENTROPY", "-DBR_SIM_DEBUG", "-fPIC", "-shared", "-std=c++17",
-                           "-ffp-contract=off", "-Wno-unused-function", "-o", so,
+                           "-ffp-contract=off", "-Wno-unused-function", "-I", os.path.join(ROOT, "include"), "-o", so,
                            os.path.join(ROOT, "tests", "sim", "br_sim.cc")])
     L = C.CDLL(so)
     L.sim_init.argtypes = [C.c_char_p, C.c_size_t, C.c_uint32]

@@ -264,7 +264,7 @@ def test_batch_of_small_streams(b200):
         got = b200.compress_batch(streams, q, w, threads=4)
         for k, x in enumerate(streams):
             assert got[k] == ora.compress(x, q, w), (q, w, k, len(x))
-    # 20 000 tiny streams (1 .. 2 000 bytes): several groups of at most 8 192 streams (br_api.cc kBatchGroupStreams)
+    # 20 000 tiny streams (1 .. 2 000 bytes): several groups of at most 8 192 streams (br_driver.h kBatchGroupStreams)
     tiny = []
     for _ in range(20000):
         n = int(rnd.choice([1, 2, 3, 7, 30, 200, 700, 2000]))
@@ -479,7 +479,7 @@ def test_q1_flush(b200):
 
 def test_q1_stream_beyond_one_device_segment(b200):
     """Quality 1 has no stream-size limit: input above one device segment (128 MiB) runs as several, a segment that
-    neither flushes nor finishes ends mid-byte and the next starts behind its pending bits (br_api.cc q1_run).
+    neither flushes nor finishes ends mid-byte and the next starts behind its pending bits (br_driver.h q1_run).
     300 MB in one call (split at multiples of the fragment size) and in 24 MiB + 1 calls (a segment every 64 MiB)."""
     from corpus import synth_web
     rng = np.random.default_rng(77)

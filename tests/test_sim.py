@@ -40,7 +40,7 @@ def test_sim_matches_oracle(sim, c):
     d = make_case(c)
     if c["q"] == 1:
         # quality 1: the stream as the device code makes it (the one-shot wrapper's empty-input and
-        # raw-stream rules live in br_api.cc)
+        # raw-stream rules live in br_driver.h)
         want = Oracle().compress_q1_stream(d, c["lgwin"])
         cap = 2 * len(d) + 100000
         out = C.create_string_buffer(cap)
@@ -72,42 +72,11 @@ def test_sim_q1_call_patterns(sim):
             assert r >= 0 and out.raw[:r] == want, (calls, w)
 
 
-def test_sim_q1_flush_segments(sim):
-    """FLUSH at quality 1: the stream is a chain of byte-aligned segments (window bits only in the first,
-    byte padding behind every flushed one): device code per segment == oracle for the whole op sequence."""
-    from corpus import synth_web
-    d = synth_web(500000, 42)
-    ora = Oracle()
-    cases = [([0, 500000], [1, 2]), ([100000, 0, 400000, 0], [1, 1, 1, 2]), ([1, 2, 3, 499994], [1, 1, 0, 2]),
-             ([200000, 150000, 150000], [0, 1, 2]), ([250000, 250000, 0], [1, 1, 2])]
-    for sizes, ops in cases:
-        for w in (16, 22):
-            want = ora.compress_q1_stream(d, w, sizes, ops)
-            got, pos, seg_calls, seg_start, header = b"", 0, [], 0, 1
-            for a, op in zip(sizes, ops):
-                if a or op == 2:
-                    seg_calls.append(a)
-                pos += a
-                if op in (1, 2):
-                    piece = d[seg_start:pos]
-                    if op == 2 and not header and not piece:
-                        got += b"\x03"
-                    elif piece or header:
-                        arr = (C.c_size_t * max(1, len(seg_calls)))(*seg_calls)
-                        cap = 2 * len(piece) + 100000
-                        out = C.create_string_buffer(cap)
-                        r = sim.sim_q1_compress_seg(w, piece, len(piece), arr if seg_calls else None, len(seg_calls), out, cap, header, op, 0, None)
-                        assert r >= 0
-                        got += out.raw[:r]
-                        header = 0
-                    seg_calls, seg_start = [], pos
-            assert got == want, (sizes, ops, w)
-
-
 def test_sim_q1_segments_mid_byte(sim):
     """Bounded-memory streaming at quality 1: the stream is cut into device segments between calls; a segment that
     neither flushes nor finishes ends mid-byte and the next one starts behind its pending bits (encode.c:1445
-    last_bytes_).  Device code per segment, stitched the way br_api.cc q1_segment does == oracle for the op sequence."""
+    last_bytes_).  Device code per segment, stitched the way brotli_b200/csrc/br_driver.h q1_segment does == oracle for the
+    op sequence (tests/test_stream_driver.py runs the driver itself)."""
     from corpus import synth_web
     d = synth_web(400000, 7) + bytes(np.random.default_rng(5).integers(0, 256, 70000, dtype=np.uint8))
     ora = Oracle()
@@ -175,73 +144,6 @@ def test_sim_fuzz_sample(sim):
             assert _fuzz_check(sim, d, q, w), (i, len(d), q, w)
     for i, d, q, w in dict_cases(20250923, 40, TABLES):
         assert _fuzz_check(sim, d, q, w), ("dict", i, len(d), q, w)
-
-
-def _sim_cuts(sim, d, q, w, hint, cuts, kinds, is_final, finish_empty=0, lgblock=0, disable_ctx=0, stream_offset=0, with_header=1):
-    sim.sim_compress_cuts.restype = C.c_long
-    sim.sim_compress_cuts.argtypes = [C.c_int, C.c_int, C.c_uint32, C.c_char_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
-                                      C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_int, C.c_uint32]
-    cp = (C.c_uint32 * max(1, len(cuts)))(*cuts)
-    ck = (C.c_uint32 * max(1, len(cuts)))(*kinds)
-    eb = (C.c_uint64 * max(1, len(cuts)))()
-    cap = len(d) + len(d) // 2 + 4096
-    out = C.create_string_buffer(cap)
-    st = np.zeros(8, np.uint32)
-    r = sim.sim_compress_cuts(q, w, hint, d, len(d), cp, ck, len(cuts), is_final, with_header, finish_empty, eb, out, cap, st.ctypes.data,
-                              lgblock, disable_ctx, stream_offset)
-    assert r >= 0
-    return out.raw[:r]
-
-
-def test_sim_flush_cuts_and_parameters(sim):
-    """The device code with the input cut by FLUSH operations (encode.c:1356, :1700), with FINISH arriving without input
-    behind a full block (encode.c:520), and with BROTLI_PARAM_LGBLOCK / DISABLE_LITERAL_CONTEXT_MODELING, against the
-    reference's CompressStream driven with the same calls."""
-    from brotli_libs import RecordedRef, ref_stream_ops
-    from corpus import synth_binary, synth_text, synth_web
-    ref = RecordedRef()
-    for d in (synth_text(400000, 3), synth_binary(600000, 5)):
-        n = len(d)
-        for q, w in ((5, 22), (9, 24), (7, 19)):
-            bs = 1 << (18 if (q >= 9 and w >= 18) else 16)
-            for sizes, ops in (([100000, 50000, n - 150000], [0, 1, 2]), ([bs, 0, n - bs, 0], [0, 1, 1, 2]), ([100, n - 100, 0], [1, 0, 2])):
-                want = ref_stream_ops(ref, d, q, w, sizes, ops)
-                pos, cuts, acc, fixed, hint = 0, [], 0, False, 0
-                for a, op in zip(sizes, ops):
-                    if not fixed and (op != 0 or acc + a >= bs):   # encode.c:1619: the size hint freezes at the first EncodeData
-                        hint, fixed = acc + a, True
-                    acc += a
-                    pos += a
-                    if op == 1 and pos > 0 and (not cuts or cuts[-1] != pos):
-                        cuts.append(pos)
-                if cuts and cuts[-1] == n:
-                    got = _sim_cuts(sim, d, q, w, hint, cuts, [1] * len(cuts), 0) + b"\x03"
-                else:
-                    got = _sim_cuts(sim, d, q, w, hint, cuts, [1] * len(cuts), 1)
-                assert got == want, (q, w, sizes, ops)
-    # quality 7..9 above 1 MiB: the pilot launch (BrParams::pilot) with the input cut by FLUSH, incl. a first block of 2 bytes
-    d = synth_web(1_400_000, 3)
-    for q, w in ((9, 24), (7, 18)):
-        for sizes, ops in (([500000, 0, 900000, 0], [1, 1, 0, 2]), ([2, 700000, 699998], [1, 1, 2])):
-            want = ref_stream_ops(ref, d, q, w, sizes, ops)
-            cuts, pos = [], 0
-            for a, op in zip(sizes, ops):
-                pos += a
-                if op == 1 and pos and (not cuts or cuts[-1] != pos):
-                    cuts.append(pos)
-            assert _sim_cuts(sim, d, q, w, sizes[0], cuts, [1] * len(cuts), 1) == want, (q, w, sizes)
-    d = synth_web(2 * 262144, 9)
-    for q, w in ((5, 22), (9, 24)):
-        want = ref_stream_ops(ref, d, q, w, [len(d), 0], [0, 2])          # FINISH without input behind full blocks
-        assert _sim_cuts(sim, d, q, w, 1 << (18 if q == 9 else 16), [], [], 1, finish_empty=1) == want
-        for lgb, dis in ((0, 1), (17, 0), (20, 1), (24, 0)):
-            prm = {}
-            if lgb:
-                prm[3] = lgb
-            if dis:
-                prm[4] = 1
-            want = ref_stream_ops(ref, d, q, w, [len(d)], [2], params=prm)
-            assert _sim_cuts(sim, d, q, w, len(d), [], [], 1, lgblock=lgb, disable_ctx=dis) == want, (q, w, lgb, dis)
 
 
 def _sim_multi(sim, streams, q, w):
@@ -373,21 +275,6 @@ def test_sim_batch_fuzz_sample(sim):
     assert checked > 100
 
 
-def test_sim_stream_offset(sim):
-    """BROTLI_PARAM_STREAM_OFFSET (encode.h:231, the sanctioned way to stitch shards into one stream, SURVEY.md 8e): no
-    window bits, poisoned distance cache (encode.c:656), dictionary distances counted from the virtual start
-    (backward_references_inc.h:94), and the first two bytes flushed on their own (encode.c:1704) -- against the reference."""
-    from brotli_libs import RecordedRef, ref_stream_ops
-    from corpus import synth_text, synth_web
-    ref = RecordedRef()
-    for d in (synth_text(300000, 4), synth_web(500000, 10)):
-        for q, w in ((5, 22), (9, 24), (6, 18)):
-            for off in (1, 1000, 1 << 20, 1 << 30):
-                want = ref_stream_ops(ref, d, q, w, [len(d)], [2], params={9: off})
-                got = _sim_cuts(sim, d, q, w, len(d), [2], [1], 1, stream_offset=off, with_header=0)
-                assert got == want, (q, w, off, len(got), len(want))
-
-
 # ---------------------------------------------------------------------------------------------------------------------
 # Qualities 2..4 (SURVEY.md 8f rank 1): slot-sorted index + br_find_quick + br_verify_run, flat metablocks at quality 2, 3
 from golden_cases import CASES_ORACLE_ONLY
@@ -433,38 +320,6 @@ def test_sim_q234_fuzz_sample(sim):
     for i, d, q, w in dict_cases(20250926, 30, TABLES):     # static-dictionary words: the shallow probe of H2 / H4
         for q2 in (2, 4):
             assert _fuzz_check(sim, d, q2, w), ("dict", i, len(d), q2, w)
-
-
-def test_sim_q234_flush_cuts(sim):
-    """Qualities 2..4 with the input cut by FLUSH operations, against the reference's CompressStream driven with the same
-    calls: input blocks of 1 << 14 bytes below quality 4 (quality.h:81), the MAX_NUM_DELAYED_SYMBOLS flush rule
-    (encode.c:1152), FINISH without input behind a full block."""
-    from brotli_libs import RecordedRef, ref_stream_ops
-    from corpus import synth_binary, synth_text
-    ref = RecordedRef()
-    for d in (synth_text(300000, 3), synth_binary(400000, 5)):
-        n = len(d)
-        for q, w in ((2, 22), (3, 18), (4, 22), (4, 12)):
-            bs = 1 << (14 if q < 4 else 16)
-            for sizes, ops in (([100000, 50000, n - 150000], [0, 1, 2]), ([bs, 0, n - bs, 0], [0, 1, 1, 2]), ([100, n - 100, 0], [1, 0, 2])):
-                want = ref_stream_ops(ref, d, q, w, sizes, ops)
-                pos, cuts, acc, fixed, hint = 0, [], 0, False, 0
-                for a, op in zip(sizes, ops):
-                    if not fixed and (op != 0 or acc + a >= bs):   # encode.c:1619: the size hint freezes at the first EncodeData
-                        hint, fixed = acc + a, True
-                    acc += a
-                    pos += a
-                    if op == 1 and pos > 0 and (not cuts or cuts[-1] != pos):
-                        cuts.append(pos)
-                if cuts and cuts[-1] == n:
-                    got = _sim_cuts(sim, d, q, w, hint, cuts, [1] * len(cuts), 0) + b"\x03"
-                else:
-                    got = _sim_cuts(sim, d, q, w, hint, cuts, [1] * len(cuts), 1)
-                assert got == want, (q, w, sizes, ops)
-    d = synth_text(4 * 65536, 9)
-    for q, w in ((2, 22), (3, 22), (4, 22)):
-        want = ref_stream_ops(ref, d, q, w, [len(d), 0], [0, 2])          # FINISH without input behind full blocks
-        assert _sim_cuts(sim, d, q, w, 1 << (14 if q < 4 else 16), [], [], 1, finish_empty=1) == want, (q, w)
 
 
 def test_sim_q234_batch_of_streams(sim):
@@ -555,24 +410,3 @@ def test_sim_q234_index_against_numpy(sim):
         assert sim.sim_debug_sort(q, 22, d, n, S.ctypes.data, seg.ctypes.data)
         assert np.array_equal(S, want_S), (q, n)
         assert np.array_equal(seg, want_seg), (q, n)
-
-
-def test_sim_flush_just_behind_a_block_boundary(sim):
-    """A FLUSH one or two bytes (up to HashTypeLength - 2) behind a block boundary leaves an input block too short to stitch
-    (hash_longest_match_quickly_inc.h:119 / hash_longest_match64_inc.h:127: num_bytes >= HashTypeLength - 1); the block behind
-    it stitches instead, and its three positions reach back across the short block into the block in front.  Their owner must
-    still commit them (br_commit_bits; found by a randomized FLUSH campaign: q3, lgwin 12, flush at 14 * 16384 + 2)."""
-    from brotli_libs import RecordedRef, ref_stream_ops
-    from corpus import synth_text
-    ref = RecordedRef()
-    d = synth_text(200000, 77)
-    n = len(d)
-    for q, w in ((3, 12), (2, 22), (4, 16), (5, 22), (7, 17)):
-        bs = 1 << (14 if q < 4 else 16)
-        for extra in (1, 2, 3, 5, 6):
-            c = 2 * bs + extra
-            want = ref_stream_ops(ref, d, q, w, [c, n - c], [1, 2])
-            assert _sim_cuts(sim, d, q, w, c, [c], [1], 1) == want, (q, w, extra)
-        c1, c2 = bs + 1, bs + 2                                    # two short blocks in a row
-        want = ref_stream_ops(ref, d, q, w, [c1, 1, n - c2], [1, 1, 2])
-        assert _sim_cuts(sim, d, q, w, c1, [c1, c2], [1, 1], 1) == want, (q, w)
